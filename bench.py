@@ -1,15 +1,15 @@
 #!/usr/bin/env python
-"""bench.py — Llama-3-8B int4 g128 QuantLinear stack on B200: bs=1 decode tok/s + 2048-token prefill TFLOP/s.
+"""bench.py — Llama-3-8B int4 g128 QuantLinear stack on H100: bs=1 decode tok/s + 2048-token prefill TFLOP/s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
 A "step" is ONE decode token through the hot path: the 224 GPTQ QuantLinear forwards of Llama-3-8B
 (32 layers x q,k,v,o,gate,up,down; BASELINE.json configs[1]) on synthetic packed weights, chained
 h -> q -> o -> gate -> down -> next layer (k, v, up are computed from the same inputs, their outputs unused: the
-reference owns no attention / norm code, SURVEY.md §1).  3.63 GB of weights are streamed per step, far more than
-the 126 MB L2, so no flush is needed between timed steps.  The prefill figure (M = 2048 through the same 224
+reference owns no attention / norm code).  3.63 GB of weights are streamed per step, far more than
+the 50 MB L2, so no flush is needed between timed steps.  The prefill figure (M = 2048 through the same 224
 layers) is measured in the same run and reported under "prefill".
 With --gpus N > 1 the stack is tensor-parallel (column shards for q,k,v,gate,up; row shards + one NCCL
 all-reduce for o and down), strong scaling.
@@ -17,6 +17,11 @@ all-reduce for o and down), strong scaling.
 --impl reference times the reference's own CPU path for this hot path (TorchAtenLinear's int4pack fused op,
 restated in oracle/gptq_oracle.py::CpuFusedLinear) on the host cores; each step is a bounded sample
 (1 of the 32 decoder layers).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed decode step and the last timed prefill pass returned
+(DIR/decode_out.npy [1, 4096], DIR/prefill_out.npy [2048, 4096], float32; at most 64 MB in all: a larger prefill
+output is a fixed, seeded sample of its rows).  Weights and inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -30,6 +35,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+DUMP_BYTES = 64 << 20  # --dump-outputs budget
 METRIC = "W4A16 g128 QuantLinear: decode tok/s + prefill TFLOPS vs HBM/TC roofline"
 CFG = dict(name="Llama-3-8B", hidden=4096, inter=14336, kv=1024, layers=32, bits=4, group_size=128)
 LINEARS = [  # name, K, N, parallel style
@@ -45,15 +51,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"],
                     tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback")
-
-
-def load_traffic():
-    """DRAM bytes measured by ncu (--set full) for one decode launch, as a ratio of its algorithmic bytes."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(p):
-        return json.load(open(p))
-    return None
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16/bf16 — not reached, an upper bound
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="datasheet")
 
 
 def algorithmic_bytes(K, N, gs, bits, M):
@@ -466,7 +465,7 @@ def extra_workloads(args, device, rank, world, peaks):
             ms, fin = time_stack(st, 1, 1, device, 20, CFG["hidden"])
             msp, _ = time_stack(st, args.prefill_tokens, 1, device, 3, CFG["hidden"])
             return {"workload": "Llama-3-8B int4 g128 act-order (desc_act=True; q|k|v and gate|up share their g_idx), "
-                                "1xB200 (BASELINE configs[2])", "decode_tok_s": 1e3 / ms,
+                                "1xH100 (BASELINE configs[2])", "decode_tok_s": 1e3 / ms,
                     "decode_frac_hbm": alg / (ms * 1e-3) / 1e9 / hbm,
                     "prefill_tflops": 2.0 * args.prefill_tokens * weights / (msp * 1e-3) / 1e12, "finite": fin}
         entry("act_order_8b", act_order)
@@ -501,7 +500,7 @@ def extra_workloads(args, device, rank, world, peaks):
             c = MIXTRAL
             shard = None if world == 4 else (0, 4)
             st = build_mixtral(device, rank, world, c["layers"], shard=shard)
-            # bytes per token per GPU: attention linears + the top-2 active experts (SURVEY 8d: 6.80 GB per token / 4)
+            # bytes per token per GPU: attention linears + the top-2 active experts (BASELINE.md §2: 6.80 GB per token / 4)
             att = sum(algorithmic_bytes(K, N, 64, 4, 1) for K, N in (
                 (c["hidden"], c["hidden"] // 4), (c["hidden"], c["kv"] // 4), (c["hidden"], c["kv"] // 4),
                 (c["hidden"] // 4, c["hidden"])))
@@ -536,16 +535,18 @@ def main():
     ap.add_argument("--with-vllm", action="store_true", help="competitors: also vLLM's Marlin build (import takes ~70 s)")
     ap.add_argument("--nccl-allreduce", action="store_true",
                     help="keep NCCL for the small decode all-reduces (default: b2q_allreduce, our one-shot kernel over "
-                         "NVLink peer memory; measured 715 vs 605 tok/s at TP-4)")
+                         "NVLink peer memory)")
     ap.add_argument("--overlap-chunks", type=int, default=1,
-                    help="N > 1 prefill: token blocks whose all-reduce overlaps the next block's GEMM (default 1 = off: "
-                         "measured SLOWER at TP-4, 17.5 vs 12.3 ms per pass, profiles/r02_tp_notes.md)")
+                    help="N > 1 prefill: token blocks whose all-reduce overlaps the next block's GEMM (default 1 = off)")
     ap.add_argument("--no-fuse", action="store_true", help="one launch per QuantLinear (224/step) instead of fusing q/k/v and gate/up")
     ap.add_argument("--decode-v2", action="store_true",
                     help="EXPERIMENTAL: decode tier v2 (b2q_decode2.cu; sets B2Q_DECODE_V2=1), result marked experimental")
     ap.add_argument("--fused-allreduce", action="store_true",
                     help="EXPERIMENTAL (N > 1): row-parallel matmul + all-reduce in one launch (b2q_decode_allreduce)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last decode step's and prefill pass's outputs as DIR/*.npy")
     args = ap.parse_args()
+    torch.manual_seed(0)  # same arguments -> same inputs, run to run
     global OVERLAP_CHUNKS
     OVERLAP_CHUNKS = args.overlap_chunks
     if args.decode_v2:
@@ -613,6 +614,9 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     ms = timed_replays(g_dec, args.steps, world, device)
+    dumps = {}
+    if args.dump_outputs and rank == 0:
+        dumps["decode_out"] = out_dec.float().cpu()
     clocks_dec = None
     ms_per_step = ms / args.steps
     toks = 1e3 / ms_per_step
@@ -646,6 +650,19 @@ def main():
     for _ in range(3):
         g_pre.replay()
     ms_pre = timed_replays(g_pre, it_pre, world, device) / it_pre
+    if args.dump_outputs and rank == 0:
+        # at most DUMP_BYTES in all: beyond that, a fixed seeded sample of the prefill rows (sorted row order)
+        rows_fit = max(1, (DUMP_BYTES - dumps["decode_out"].numel() * 4) // (out_pre.shape[1] * 4))
+        if out_pre.shape[0] <= rows_fit:
+            dumps["prefill_out"] = out_pre.float().cpu()
+        else:
+            pick = torch.randperm(out_pre.shape[0], generator=torch.Generator().manual_seed(0))[:rows_fit].sort().values
+            dumps["prefill_out"] = out_pre[pick.to(out_pre.device)].float().cpu()
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in dumps.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.numpy())
     sampler.stop_flag = True
     sampler.join(timeout=2)
     clocks = sampler.result()
@@ -682,7 +699,7 @@ def main():
             arms = ("b2q", "marlin_ref", "marlin_vllm") if args.with_vllm else ("b2q", "marlin_ref")
             competitors = _comp.run(arms, Ms=(1, 16, 64, 2048), nlayers=CFG["layers"], stack=True, verbose=False)
             competitors["note"] = ("same box, same packed checkpoint tensors; marlin_ref = the reference's own "
-                                   "gptqmodel_ext/marlin compiled for sm_100a by baseline/build_marlin.py; per-shape us = "
+                                   "gptqmodel_ext/marlin compiled for sm_90a by oracle/build_marlin.py; per-shape us = "
                                    "mean over a CUDA graph walking >= 600 MB of distinct layers; stack = 224 separate "
                                    "launches per step for every arm (this repo's headline additionally fuses q|k|v and gate|up)")
         except Exception as e:  # noqa: BLE001
@@ -701,9 +718,7 @@ def main():
     phase("cpu baseline done")
     if rank == 0:
         achieved = alg_bytes_step / (ms_per_step * 1e-3) / 1e9  # GB/s per GPU
-        tr = load_traffic()
         n_launch = n_lin if args.no_fuse else 4 * args.layers
-        traffic = (tr["decode_kernel"]["ratio"] * alg_bytes_step / n_launch) if tr else None
         line = {
             "metric": METRIC, "value": toks, "unit": "tok/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong",
@@ -714,7 +729,7 @@ def main():
                                                (", decode all-reduce: b2q_allreduce (P2P one-shot kernel), "
                                                 "prefill all-reduce: NCCL" if P2P_AR is not None
                                                 else ", all-reduce: NCCL")),
-                "l2": "3.63 GB of distinct weights per step >> 126 MB L2: no flush needed between timed steps",
+                "l2": "3.63 GB of distinct weights per step >> 50 MB L2: no flush needed between timed steps",
                 "timing": "CUDA graph of the whole step, CUDA events around K replays, max over ranks",
                 **({"experimental": [f for f, on in (("decode-v2", args.decode_v2),
                                                      ("fused-allreduce", FUSED_AR is not None)) if on]}
@@ -730,22 +745,15 @@ def main():
                 "bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                 "frac": achieved / peaks["hbm_gbs"], "peak_source": peaks["source"],
                 "algorithmic_bytes_per_launch": alg_bytes_step / n_launch,
-                "traffic": None if args.decode_v2 else traffic,  # the ncu capture is of the default kernel
-                "traffic_note": "average per launch = measured DRAM/algorithmic ratio of the ncu --set full capture "
-                                "(profiles/r02_decode_ncu.txt: 30,317,568 B DRAM vs 30,539,776 B algorithmic for the "
-                                "4096x14336 launch) x algorithmic bytes per launch",
             },
             "prefill": {
                 "tokens": Mp, "ms_per_pass": ms_pre, "tflops": tflops, "iters": it_pre,
                 "tokens_per_s": Mp / (ms_pre * 1e-3),
-                "roofline": {"kernel": "gemm2p_kernel (persistent CTA pairs, tcgen05.mma.cta_group::2 + TMA, TMEM accumulators)", "bound": "tensor",
+                "roofline": {"kernel": "gemm_kernel (wgmma + TMA, register accumulators, q|k|v and gate|up in one launch)",
+                             "bound": "tensor",
                              "achieved": tflops / world, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                              "frac": tflops / world / peaks["tflops_sustained"],
-                             "peak_note": "sustained cuBLAS bf16 (kernel timed inside a long step); burst peak "
-                                          f"{peaks['tflops_burst']}",
-                             "traffic": (tr or {}).get("gemm2p_kernel", {}).get("dram_bytes"),
-                             "traffic_note": "DRAM bytes of ONE 4096x4096 M=2048 launch (ncu --set full, "
-                                             "profiles/r02_gemm2p_ncu.txt); tensor-bound kernel"},
+                             "peak_note": f"dense fp16 peak ({peaks['source']}); burst peak {peaks['tflops_burst']}"},
                 "e2e_ms_per_pass": pre_e2e_ms,
                 "e2e_tokens_per_s": Mp / (pre_e2e_ms * 1e-3),
             },

@@ -1,4 +1,4 @@
-"""gptqmodel_b200 — B200-native (sm_100a) GPTQ W4A16/W8A16 QuantLinear hot path.
+"""gptqmodel_b200 — H100-native (sm_90a) GPTQ W4A16/W8A16 QuantLinear hot path.
 
 Public API:
     B200QuantLinear   drop-in QuantLinear (reference contract: gptqmodel/nn_modules/qlinear)

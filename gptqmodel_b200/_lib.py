@@ -53,7 +53,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python __graft_entry__.py` or `make -C gptqmodel_b200/csrc` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU/PyTorch fallback."
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU/PyTorch fallback."
         )
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():

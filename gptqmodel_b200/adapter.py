@@ -1,6 +1,6 @@
 """LoRA adapter for the QuantLinear epilogue hook (`forward()` calls `adapter.apply(x=x, out=out)`).
 
-Same interface and arithmetic as the reference's `Lora` (/root/reference/gptqmodel/adapter/adapter.py:116-260):
+Same interface and arithmetic as the reference's `Lora` (gptqmodel/adapter/adapter.py:116-260):
 ``out += (x @ lora_A) @ lora_B`` with ``lora_A [in_features, r]`` and ``lora_B [r, out_features]`` (the transposes of
 PEFT's ``<module>.lora_A.weight [r, K]`` / ``<module>.lora_B.weight [N, r]``), matrices moved to the activations' dtype
 and device on first use.  The two skinny GEMMs are plain dense library GEMMs (cuBLAS through torch): they are not the

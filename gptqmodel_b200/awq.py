@@ -1,10 +1,10 @@
-"""AWQ (FORMAT.GEMM) front-end onto the same B200 kernels (SURVEY.md §8 row f3).
+"""AWQ (FORMAT.GEMM) front-end onto the same B200 kernels.
 
 An AWQ GEMM-format checkpoint stores ``qweight int32 [K, N/8]`` packed along the OUTPUT dimension with the nibbles of
 every word interleaved (nibble i holds logical column 8c + [0, 2, 4, 6, 1, 3, 5, 7][i]), ``qzeros int32 [G, N/8]`` packed
 the same way and ``scales fp16 [G, N]``; its dequantisation is ``(q - z) * scale`` with the true zero-point
-(/root/reference/gptqmodel/nn_modules/qlinear/__init__.py:1634-1668,
-/root/reference/gptqmodel/quantization/awq/utils/packing_utils.py:9-10, 106-121).  That is exactly the arithmetic of a
+(gptqmodel/nn_modules/qlinear/__init__.py:1634-1668,
+gptqmodel/quantization/awq/utils/packing_utils.py:9-10, 106-121).  That is exactly the arithmetic of a
 GPTQ v2 layer, so one exact integer re-packing at load time (``awq_gemm_to_gptq``) lets the fragment-major prepack and
 every kernel of this package serve AWQ models unchanged — the route the reference's own AwqSwordfishLinear / AwqMarlin
 take (qlinear/swordfish.py:358-394, 565-606).

@@ -1,4 +1,4 @@
-"""Build libb2q.so in-tree for sm_100a (`python gptqmodel_b200/build.py`, or `__graft_entry__.build()`)."""
+"""Build libb2q.so in-tree for sm_90a (`python gptqmodel_b200/build.py`, or `__graft_entry__.build()`)."""
 import os
 import subprocess
 import sys

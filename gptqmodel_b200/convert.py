@@ -1,11 +1,11 @@
-"""Swap the nn.Linear modules of a model for B200 QuantLinears (the caller side of the hot path, SURVEY.md §8 f2).
+"""Swap the nn.Linear modules of a model for B200 QuantLinears (the caller side of the hot path).
 
-The reference does this in `make_quant` / `create_quant_module` (/root/reference/gptqmodel/utils/model.py:475-649): walk
+The reference does this in `make_quant` / `create_quant_module` (gptqmodel/utils/model.py:475-649): walk
 the model, replace every targeted `nn.Linear` by the selected QuantLinear class, load the packed tensors, `post_init()`.
 `replace_linears` is that walk.  `rtn_grid` + `quantize_linear` build the packed tensors from float weights with a plain
 round-to-nearest grid (per-group min/max or abs-max) through the device-side packer — enough to turn any float model into
 a GPTQ-layout model for tests and synthetic benchmarks; it is NOT a replacement for the reference's calibrated GPTQ / AWQ
-quantisers (out of scope, DESIGN.md §7).
+quantisers (out of scope).
 """
 from __future__ import annotations
 

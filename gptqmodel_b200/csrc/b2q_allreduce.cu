@@ -1,5 +1,5 @@
 // b2q_allreduce.cu — latency-optimised one-shot all-reduce(sum) of a small vector over NVLink peer memory, for the
-// row-parallel QuantLinear output at decode time (8-16 KB per call, 2 calls per decoder layer: SURVEY.md §8e).
+// row-parallel QuantLinear output at decode time (8-16 KB per call, 2 calls per decoder layer).
 //
 // Every rank owns one SYMMETRIC buffer (same layout on all GPUs, peers mapped through torch's symmetric-memory
 // rendezvous): data[2 slots][world][max_elems] (16-bit) followed by flags[2 slots][world] (u32).
@@ -10,7 +10,7 @@
 // seq lives in device memory and only grows, so nothing is ever reset: CUDA-graph replay safe.  Slots alternate with
 // seq, so a fast rank's call n+1 never overwrites data a slow rank is still reading for call n.
 // The flag wait is bounded (2 s of %globaltimer): a dead peer leaves 1 + its rank in seq[1] instead of hanging the GPU.
-// One CTA, no NCCL, ~4 us instead of NCCL's LL all-reduce; the reference has no collective at all (SURVEY §2c).
+// One CTA, no NCCL; the reference has no collective at all.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(256) allreduce_kernel(ARPeers peers, T* inout,
                                                         int max_elems, size_t flag_offset, uint32_t* seq_ptr) {
   // programmatic dependent launch on both sides: the NEXT kernel of the stream (a decode launch) may start its weight
   // prefetch now, and this kernel was itself launched while the matmul that produces `inout` was still running — a plainly
-  // launched all-reduce between two PDL kernels serialised the whole chain (TP-2: 651 tok/s against 800 on one GPU)
+  // launched all-reduce between two PDL kernels serialised the whole chain (a TP-2 decode step slower than one GPU)
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   const uint32_t seq = *seq_ptr;

@@ -24,20 +24,35 @@ static int env_int(const char* name, int dflt) {
 static EnvCfg read_env() {
   EnvCfg c;
   c.disable_pdl = env_int("B2Q_DISABLE_PDL", 0);
-  c.gemm_1cta = env_int("B2Q_GEMM_1CTA", 0);
   c.midm = env_int("B2Q_MIDM", 1);
   c.decode_blocks_m = env_int("B2Q_DECODE_BLOCKS_M", 0);
   c.decode_groups2 = env_int("B2Q_DECODE_GROUPS", 1) == 2;
   c.decode_v2 = env_int("B2Q_DECODE_V2", -1);
   c.decode2_gw = env_int("B2Q_DECODE2_GW", 0);
   c.decode2_ks = env_int("B2Q_DECODE2_KS", 0);
-  c.decode2_xtma = env_int("B2Q_DECODE2_XTMA", 0);  // LDG staging measured faster (799.6 vs 789.1 tok/s, profiles/r02_decode_notes.md)
+  c.decode2_xtma = env_int("B2Q_DECODE2_XTMA", 0);
   c.decode2_fastsync = env_int("B2Q_DECODE2_FASTSYNC", 0);
-  c.gemm2_persist = env_int("B2Q_GEMM2_PERSIST", 1);
-  c.gemm2_dqw = env_int("B2Q_GEMM2_DQW", 8) == 4 ? 4 : 8;
   c.midm_ks = env_int("B2Q_MIDM_KS", 0);
   c.midm_dqg1 = env_int("B2Q_MIDM_DQG1", 0);
   return c;
+}
+
+int num_sms() {
+  static int cache[32] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 32) {
+    (void)cudaGetLastError();
+    return 132;
+  }
+  if (cache[dev] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      (void)cudaGetLastError();
+      n = 132;
+    }
+    cache[dev] = n < 160 ? n : 160;  // the decode all-reduce keeps flag columns for at most 160 CTAs per launch
+  }
+  return cache[dev];
 }
 
 static EnvCfg g_env = read_env();  // once, at library load
@@ -349,7 +364,7 @@ int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const vo
     if (e != 0) return e;
     xa = workspace;
   }
-  return check_cuda(launch_gemm2_multi(a, xa, nsets, packed, scales, qzeros, bias, out, N), "b2q_gemm_multi");
+  return check_cuda(launch_gemm_multi(a, xa, nsets, packed, scales, qzeros, bias, out, N), "b2q_gemm_multi");
 }
 
 int b2q_gemm(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
@@ -361,7 +376,6 @@ int b2q_gemm(const void* x, const void* packed, const void* scales, const int32_
   if (M == 0) return 0;
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, M, K, N, bits, group_size, dtype, workspace,
                        workspace_bytes, stream);
-  if (env().gemm_1cta) a.tune_ks = -1;  // debugging / A-B measurements: keep the single-CTA tier
   return check_cuda(launch_gemm(a), "b2q_gemm");
 }
 
@@ -375,8 +389,8 @@ int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t*
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, M, K, N, bits, group_size, dtype, workspace,
                        workspace_bytes, stream);
   if (decode_supported(a)) return check_cuda(launch_decode(a), "b2q_mm(decode)");
-  // 9 <= M <= B2Q_DECODE_BLOCKS_M (default off): passes of the decode tier over blocks of 8 rows, the round-1 answer to
-  // the padded single-CTA tier's 28 us; superseded by the small-batch tier (b2q_midm.cu), kept for A/B measurements
+  // 9 <= M <= B2Q_DECODE_BLOCKS_M (default off): passes of the decode tier over blocks of 8 rows, an earlier answer to
+  // the padded 128-token tile's waste; superseded by the small-batch tier (b2q_midm.cu), kept for A/B measurements
   {
     MmArgs a8 = a;
     a8.M = 8;
@@ -393,7 +407,6 @@ int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t*
     }
   }
   if (M == 1 && bits == 8 && K % 128 == 0) return check_cuda(launch_gemv(a), "b2q_mm(gemv)");
-  if (env().gemm_1cta) a.tune_ks = -1;
   return check_cuda(launch_gemm(a), "b2q_mm(gemm)");
 }
 

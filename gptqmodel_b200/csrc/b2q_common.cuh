@@ -1,7 +1,7 @@
-// b2q_common.cuh — shared device helpers for the B200 (sm_100a) GPTQ QuantLinear kernels.
+// b2q_common.cuh — shared device helpers for the H100 (sm_90a) GPTQ QuantLinear kernels.
 //
 // Prepacked weight layouts ("B2Q tiles", produced by b2q_prepack.cu from the checkpoint layout
-// qweight int32 [K*bits/32, N] of /root/reference/gptqmodel/nn_modules/qlinear/__init__.py:827-865):
+// qweight int32 [K*bits/32, N] of GPTQModel's gptqmodel/nn_modules/qlinear/__init__.py:827-865):
 //
 //   4-bit:  uint4 T4[K/64][N/16][32]      one warp-wide 512-byte row = 16 output features x 64 k
 //   8-bit:  uint4 T8[K/32][N/32][2][32]   one uint4 = 16 consecutive k of ONE output feature n
@@ -15,7 +15,7 @@
 // half2(1024+16q) of (g+8, k+0..1), and the same two masks on (w >> 8) give k+2..3: FOUR LOP3 (+1 shift) turn a
 // word into the four A-operand registers of one mma.sync.m16n8k16 (decode tier: rows g / g+8, the k permutation is
 // shared with the activation fragment), and the same registers are K-consecutive pairs of ONE feature row, so the
-// tcgen05 GEMM tier stores them as 16-byte K-major shared-memory chunks.  Rows g carry the magic bias 1024, rows g+8
+// wgmma GEMM tiers store them as 16-byte K-major shared-memory chunks.  Rows g carry the magic bias 1024, rows g+8
 // carry 16*(64+q): one bias class per output row, removed once per group with the activation sum.
 // A CTA tile of 128 features x 64 k is ONE contiguous 4 KB block for cp.async.bulk.
 // With act-order the rows are first sorted by group (k' -> original row perm[k']) so groups are contiguous.
@@ -48,38 +48,21 @@ __device__ __forceinline__ uint32_t lop3_and_or(uint32_t a, uint32_t mask, uint3
   return r;
 }
 
-// d = a(f16 half of reg, selected by H) * b(f16 half) + c(f32)  -> SASS FHFMA on sm_100a
+// d = a(16-bit half of reg) * b(16-bit half) + c(f32) with ONE rounding.  Hopper has no mixed-precision FMA: both halves
+// are widened exactly to f32 and a product of two 11-bit (fp16) or 8-bit (bf16) significands is exact in f32, so
+// fma.rn.f32 of the widened operands is the same operation.
 __device__ __forceinline__ float fhfma_lo(uint32_t a2, uint32_t b2, float c) {
-  float d;
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al, ah}, %1; mov.b32 {bl, bh}, %2;\n"
-      "  fma.rn.f32.f16 %0, al, bl, %3; }"
-      : "=f"(d)
-      : "r"(a2), "r"(b2), "f"(c));
-  return d;
+  return fmaf(__low2float(*reinterpret_cast<const __half2*>(&a2)), __low2float(*reinterpret_cast<const __half2*>(&b2)), c);
 }
 __device__ __forceinline__ float fhfma_hi(uint32_t a2, uint32_t b2, float c) {
-  float d;
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al, ah}, %1; mov.b32 {bl, bh}, %2;\n"
-      "  fma.rn.f32.f16 %0, ah, bh, %3; }"
-      : "=f"(d)
-      : "r"(a2), "r"(b2), "f"(c));
-  return d;
+  return fmaf(__high2float(*reinterpret_cast<const __half2*>(&a2)), __high2float(*reinterpret_cast<const __half2*>(&b2)),
+              c);
 }
 __device__ __forceinline__ float fbfma_lo(uint32_t a2, uint32_t b2, float c) {
-  float d;
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al, ah}, %1; mov.b32 {bl, bh}, %2;\n"
-      "  fma.rn.f32.bf16 %0, al, bl, %3; }"
-      : "=f"(d)
-      : "r"(a2), "r"(b2), "f"(c));
-  return d;
+  return fmaf(__uint_as_float(a2 << 16), __uint_as_float(b2 << 16), c);
 }
 __device__ __forceinline__ float fbfma_hi(uint32_t a2, uint32_t b2, float c) {
-  float d;
-  asm("{ .reg .b16 al, ah, bl, bh; mov.b32 {al, ah}, %1; mov.b32 {bl, bh}, %2;\n"
-      "  fma.rn.f32.bf16 %0, ah, bh, %3; }"
-      : "=f"(d)
-      : "r"(a2), "r"(b2), "f"(c));
-  return d;
+  return fmaf(__uint_as_float(a2 & 0xFFFF0000u), __uint_as_float(b2 & 0xFFFF0000u), c);
 }
 
 // ---- mbarrier ----------------------------------------------------------------------------------
@@ -127,64 +110,6 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 }
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
-}
-
-// ---- tcgen05 -----------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{ .reg .pred p; setp.ne.b32 p, %4, 0;\n"
-      "  tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p; }"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B, rows of 128 bytes, 8-row atoms 1024 B apart.
-// Bit layout (cute/arch/mma_sm100_desc.hpp SmemDescriptor): [0,14) addr>>4, [16,30) LBO>>4,
-// [32,46) SBO>>4, [46,48) version=1, [61,64) layout (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16 instruction descriptor: c=f32, a/b format (0 f16, 1 bf16), both K-major, N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int fmt, int M, int N) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
 }
 
 // ---- bounded spin on a flag another GPU writes (peer-memory all-reduce kernels) -------------------

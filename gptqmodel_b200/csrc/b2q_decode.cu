@@ -1,10 +1,9 @@
 // b2q_decode.cu — decode tier for 4-bit weights: out[M, N] = x[M, K] @ dequant(W) for M <= 8 (batch-1 decode and
 // small speculative / multi-sequence batches), HBM-bound.
 //
-// SURVEY.md §8(d): 8,732,672 algorithmic bytes for 4096x4096 g128 at M=1; the roofline is the HBM copy bandwidth.
-// The first version of this tier multiplied on the CUDA cores (fma.rn.f32.f16, kept in b2q_gemv.cu for 8-bit); ncu
-// showed it issue-bound (156 warp-instructions per 1024 weights, profiles/r01_gemv_fhfma_v1.txt).  This version
-// needs ~27:
+// 8,732,672 algorithmic bytes for 4096x4096 g128 at M=1 (BASELINE.md §2); the roofline is the HBM copy bandwidth.
+// Multiplying on the CUDA cores (as b2q_gemv.cu does for 8-bit) is issue-bound: ~156 warp-instructions per 1024
+// weights.  This tier needs ~27:
 //  * the prepacked T4 layout stores every 32-bit word as the four A-operand registers of one
 //    mma.sync.m16n8k16 (16 features x 16 k): 4 LOP3 + 1 SHF produce them as exact 1024+q / 1024+16q halves, with
 //    NO per-weight scaling, zero-point subtraction or conversion;
@@ -52,7 +51,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   const int g = lane >> 2, t = lane & 3;
   // The CTA's warps form `ngroups` independent groups (1 or 2); a group owns whole tiles (group-strided over the
   // launch) and its `gw` warps split the k-quads of a tile.  With 2 groups, one group's tile epilogue (barrier + cross-
-  // warp reduction, ~0.5 us of mostly latency) overlaps the other group's main loop on the same SM.
+  // warp reduction, mostly latency) overlaps the other group's main loop on the same SM.
   const int gw = nwarps / ngroups;              // warps per group
   const int grp = warp / gw, wg = warp - grp * gw;
   const int C = gridDim.x * ngroups;            // tile stride of a group
@@ -151,7 +150,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   if (PERM) prefetch_inverse_perm(perm + K, K);
   // zero the token columns >= M of the block sums once (read by the fix-up of lanes whose columns are padding): own shared
   // memory, nothing to wait for — everything between griddepcontrol.wait and the first main-loop iteration is on the critical
-  // path of every launch (profiles/r02_actorder_notes.md)
+  // path of every launch
   const bool OWN = !PERM && ngroups == 1;  // per-warp staging (stage_x_own_quads): no CTA barrier before the main loop
   if (OWN) {
     zero_own_xsum_padding(xsum, M, nq, wg, gw);
@@ -167,8 +166,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
 
   // ---- 2. stage x[m, k-range] (act-order gather fused) + per-(64 k block, token) sums, ONCE ------
   // A thread's loads (up to SX_UNROLL x 16 bytes, K = 14336 needs 3.5 per thread) are all issued BEFORE the first is
-  // consumed: the rolled loop paid one dependent L2 round trip per iteration (2.6 us of the 11 us down_proj launch,
-  // profiles/r02_decode_notes.md).
+  // consumed: a rolled loop pays one dependent L2 round trip per iteration.
   if (MOE && S.moe == 3) {
     stage_x_own_quads<T, true>(x, sx, xsum, 1, K, q0, nq, wg, gw, kspan);
   } else if (OWN) {
@@ -220,7 +218,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
 
   // ---- 3. loop over this CTA's tiles; inside a tile the warps split the k-quads --------------------
   // All loop-carried addresses are 32-bit shared-window addresses / running global pointers computed ONCE here:
-  // the first version recomputed them per quad (~80 of 220 SASS instructions, profiles/r01_decode_r1c.txt).
+  // recomputing them per quad costs about a third of the loop's instructions.
   constexpr float ZSYM = 8.f;
   const uint32_t nrank = cluster_nctarank();
   const uint32_t ring_a = smem_u32(ring) + lane * 16;
@@ -315,8 +313,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     }
 
     // ---- tile epilogue: warps -> CTA through (double-buffered) smem, one barrier per tile ---------
-    // (two decoupled variants were measured and were slower: "last warp to arrive reduces" and "rotating reducer
-    //  warp on a split arrive/sync named barrier" — profiles/r01_decode_notes.md)
+    // (decoupled variants — "last warp to arrive reduces", "rotating reducer warp on a split arrive/sync named
+    //  barrier" — add synchronisation without removing the barrier's latency)
     // tot[ftl][c]: feature nt*32 + ftl*16 + g (+8 if c >= 2), token 2t + (c & 1)
     if (ti < 5) stamp(4 + 2 * ti);
     float* rbuf = red + (grp * 2 + (ti & 1)) * gw * 256;
@@ -440,10 +438,10 @@ static size_t decode_smem(int M, int warps, int qpc, int max_tiles, int nst) {
          (size_t)2 * warps * 256 * 4 + (size_t)max_tiles * 256 * 4 + (size_t)warps * DEC_STAGES * 8 + 16;
 }
 
-// Pick (C tile-columns, ks split-K ranks, warps) minimising the critical path in "quads per warp" on ~148 CTAs.
+// Pick (C tile-columns, ks split-K ranks, warps) minimising the critical path in "quads per warp" on one CTA per SM.
 static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
   const int quads = a.K / 128;
-  const int SMS = 148;
+  const int SMS = num_sms();
   double best_cost = 1e30;
   bool found = false;
   const bool two_groups = env().decode_groups2 != 0;
@@ -462,7 +460,7 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
       if (C * ngroups > NT) C = (NT + ngroups - 1) / ngroups;
       if (C < 1) C = 1;
       const int max_tiles = (NT + C * ngroups - 1) / (C * ngroups);  // per group
-      // ring depth 4 when it fits, else 2 (measured: no loss at 2 stages, profiles/r01_decode_notes.md)
+      // ring depth 4 when it fits, else 2
       int stl = 2;
       size_t smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles * ngroups : 0, 4);
       if (smem > 200 * 1024) {
@@ -471,8 +469,8 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
       }
       if (smem > 200 * 1024) continue;
       const int qpw = (qpc + gwarps - 1) / gwarps;  // quads per warp per tile
-      // calibrated on the B200 sweep (profiles/r01_decode_notes.md): per tile = quads/warp + barrier epilogue,
-      // split-K adds a cluster barrier + DSMEM pass, fewer warps hide less latency
+      // relative cost in units of one quad per warp: per tile = quads/warp + barrier epilogue, split-K adds a cluster
+      // barrier + DSMEM pass, fewer warps hide less latency (the weights are heuristic, not fitted to one GPU)
       const double cost =
           (double)max_tiles * (qpw + 0.35) / ngroups + (ks > 1 ? 0.6 : 0.0) + (16 - warps) * 0.04 * max_tiles * qpw;
       if (cost < best_cost) {
@@ -535,17 +533,18 @@ bool decode_supported(const MmArgs& a) {
 int launch_decode2_sets(const MmArgs& a, const DecSets& sets);  // b2q_decode2.cu (experimental), -2 = no configuration
 
 static int launch_decode_sets(const MmArgs& a, const DecSets& sets) {
-  // Kernel choice (same-box A/B of every Llama-3-8B launch shape, profiles/r02_decode_v1_v2_sweep.log): launches whose CTAs
-  // walk SEVERAL 32-feature tiles (more tiles than SMs: fused q|k|v 192, gate|up 896 tiles) run on decode2_kernel — warps
-  // park their partial sums and the CTA meets once, instead of a CTA barrier + reduction per tile (6.5 vs 8.5 us and
-  // 18.8 vs 19.9 us); single-tile launches (o_proj, down_proj: 128 tiles) keep decode_kernel, whose one reduction is
-  // cheaper (4.8 vs 5.5 us, 11.2 vs 12.5 us).  B2Q_DECODE_V2=1 / 0 forces one kernel for A/B runs.
+  // Kernel choice per launch shape: launches whose CTAs walk SEVERAL 32-feature tiles (more tiles than SMs: fused q|k|v,
+  // gate|up) run on decode2_kernel with one 16-warp group and no split-K — warps park their partial sums and the CTA meets
+  // once; the others keep decode_kernel.  Measured on an H100 80GB HBM3 (700 W limit, power-capped; results/h100_bench.json):
+  // Llama-3-8B decode 588 tok/s with this choice, 528 with decode_kernel everywhere, 604 with decode2_kernel everywhere —
+  // but decode2_kernel everywhere dropped the Llama-3-70B TP-8 shard stack from 372 to 277 tok/s and Mixtral TP-4 from 647
+  // to 607, so it is not the default.  B2Q_DECODE_V2=1 / 0 forces one kernel for A/B runs.
   {
     const int mode = env().decode_v2;  // -1 auto, 0 never, 1 always
     const int NT = sets.tile_end[sets.nsets - 1];
-    if (mode == 1 || (mode < 0 && NT > 148 && a.tune_ks <= 0 && a.tune_warps <= 0)) {
+    if (mode == 1 || (mode < 0 && NT > num_sms() && a.tune_ks <= 0 && a.tune_warps <= 0)) {
       MmArgs a2 = a;
-      if (mode < 0) {  // the configuration that won the sweep: no split-K, one 16-warp group
+      if (mode < 0) {  // one 16-warp group, no split-K
         a2.tune_ks = 1;
         a2.tune_warps = 16;
       }
@@ -576,7 +575,7 @@ static int launch_decode_sets(const MmArgs& a, const DecSets& sets) {
 // two decode kernels; everything else takes decode2_kernel's epilogue.  -2 = not applicable.
 int launch_decode1_allreduce(const MmArgs& a, const DecSets& sets, const DecodeAR& ar) {
   const int NT = sets.tile_end[sets.nsets - 1];
-  if (NT > 148 || a.perm != nullptr) return -2;
+  if (NT > num_sms() || a.perm != nullptr) return -2;
   MmArgs a1 = a;
   a1.tune_ks = 1;
   DecodeCfg c;
@@ -643,8 +642,8 @@ int launch_decode_multi(const MmArgs& a, int nsets, const void* const* packed, c
 }
 
 // ---- MoE decode: one token, top_k experts chosen on the device (DecSets::moe; b2q_moe_decode_*) -------------------------
-// The grouped small-batch kernels (b2q_midm.cu MODE 1 / 2) serve a single token at ~1 TB/s (tcgen05 tiles of >= 16 token
-// columns, 56 - 128 CTAs); the decode tier streams the same bytes 2 - 3x faster.  gate | up: the 2 * top_k (expert, w1 | w3)
+// The grouped small-batch kernels (b2q_midm.cu MODE 1 / 2) pad a single token to MMA tiles of >= 16 token columns; the
+// decode tier streams the same bytes without that padding.  gate | up: the 2 * top_k (expert, w1 | w3)
 // matrices are virtual sibling sets of ONE decode launch over the same activations.  down: a cluster of top_k CTAs per tile
 // column, rank r multiplying pair r's activations with ITS expert's w2; the DSMEM reduction applies the routing weights.
 static void moe_strides(DecSets& sets, int K, int N, int group_size) {
@@ -711,7 +710,7 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
   c.warps = DEC_MAX_WARPS;
   c.ngroups = 1;
   c.qpc = a.K / 128;  // a rank's k-range is its expert's whole K
-  c.C = 148 / top_k;
+  c.C = num_sms() / top_k;
   if (c.C > NT) c.C = NT;
   c.max_tiles = (NT + c.C - 1) / c.C;
   c.stl = 2;

@@ -29,8 +29,8 @@ __device__ __forceinline__ void mma_16816<__nv_bfloat16>(float (&d)[4], const ui
 // One "quad" = 128 k x 32 features = two contiguous 1 KB pieces of T4 (k-blocks 2q and 2q+1, feature tiles 2nt and
 // 2nt+1).  Each warp owns a private ring of DEC_STAGES quad buffers in shared memory, filled by cp.async.bulk
 // (UBLKCP) and tracked by one mbarrier per stage: up to DEC_STAGES * 2 KB per warp are in flight with no register
-// cost, which is what keeps > 100 KB per SM outstanding (the first, register-prefetch version of this kernel kept
-// 2 KB per warp in flight and topped out at ~3 TB/s incremental: profiles/r01_decode_notes.md).
+// cost, which is what keeps > 100 KB per SM outstanding (a register-prefetch ring keeps only 2 KB per warp in flight,
+// too little to cover HBM latency).
 constexpr int DEC_STAGES = 4;  // maximum ring depth; the launch picks 4 or 2 stages (`stl` = log2) to fit shared memory
 constexpr int DEC_QUAD_BYTES = 2048;
 
@@ -65,8 +65,8 @@ __device__ __forceinline__ void issue_quad(uint32_t dst, uint32_t bar, const uin
 // by one launch: the 32-feature tiles of all sets form one index space (tile_end = running totals).
 // ---- act-order activation staging -------------------------------------------------------------------------------------
 // `perm` (ABI v3) is int32 [2K]: perm[0:K] the sorted-by-group order (x'[k'] = x[perm[k']]), perm[K:2K] its inverse.
-// Round 2 gathered x[perm[k']] with one 2-byte global load per element: 4096 .. 14336 uncoalesced requests per CTA and
-// token, ~2 .. 7 us of LSU time per launch (act-order decode 620 vs 802 tok/s, profiles/r02_bench_n1.json).  Here every
+// Gathering x[perm[k']] with one 2-byte global load per element costs 4096 .. 14336 uncoalesced requests per CTA and
+// token.  Here every
 // CTA reads x and the INVERSE permutation with coalesced 16-byte loads and scatters the halves into the shared staging
 // buffer (sx[m][inv[k] - k0] = x[m][k] for the sorted positions this CTA owns): 8x fewer global requests, the scattered
 // accesses hit shared memory banks instead.  The per-(64-k block, token) sums are taken from shared memory afterwards.
@@ -149,7 +149,7 @@ __device__ __forceinline__ void stage_x_act_order(const T* __restrict__ x, const
 // lanes x 16 bytes per quad and token) and their 64-k block sums, so only the WARP synchronises between the load of x and its
 // first mma — the CTA-wide loop it replaces made every warp wait at a CTA barrier for the slowest L2 round trip of the CTA.
 // Everything between griddepcontrol.wait and the first main-loop iteration is on the critical path of every launch
-// (profiles/r02_actorder_notes.md: trimming it moved the whole Llama-3-8B decode step by 5 + 4 %).
+// (a few percent of the whole Llama-3-8B decode step).
 __device__ __forceinline__ void zero_own_xsum_padding(float* xsum, int M, int nq, int wg, int gw) {
   // token columns >= M of this warp's block sums (read by the fix-up of lanes whose columns are padding); before the wait
   const int lane = threadIdx.x & 31;

@@ -1,14 +1,14 @@
-// b2q_decode2.cu — second generation of the 4-bit decode tier (M <= 8).  GPU-validated in round 2 (the whole parity suite
-// passes with it forced on: profiles/r02_ab_experimental.json) and selected per launch shape by launch_decode_sets
+// b2q_decode2.cu — second generation of the 4-bit decode tier (M <= 8).  The whole parity suite passes with it forced on
+// (B2Q_DECODE_V2=1); it is selected per launch shape by launch_decode_sets
 // (b2q_decode.cu): multi-tile launches run here, single-tile launches on decode_kernel.
 //
 // Same data path as b2q_decode.cu (fragment-major T4 tiles -> per-warp cp.async.bulk ring -> mma.sync on raw
 // bias+q operands -> per-group fp32 fix-up, cluster split-K through distributed shared memory); what changes is
-// everything AROUND the main loop, which the round-1 timeline (profiles/r01_decode_notes.md) showed to cost as much as
-// the loop itself:
+// everything AROUND the main loop, which a phase timeline of the first kernel (tools/trace_decode.py) shows to cost as
+// much as the loop itself:
 //  * no per-tile epilogue: a warp parks its partial sums of a finished tile in its own slice of shared memory
 //    (tokens < M only: 128 B per warp and tile at M = 1) and moves on; the CTA meets ONCE, after its last tile, and
-//    reduces all tiles together.  v1 paid a CTA barrier + a 16-partial reduction (~0.5 us, mostly latency) per tile,
+//    reduces all tiles together.  v1 paid a CTA barrier + a 16-partial reduction (mostly latency) per tile,
 //    3-7 times per launch;
 //  * because nothing synchronises the warps between tiles any more, the warps of a CTA can form independent groups
 //    of `gw` warps that walk different tiles (gw = 16, 8, 4 ...): the launch picks (split-K ranks, warps, gw)
@@ -24,11 +24,11 @@
 
 namespace b2q {
 
-constexpr int DEC_AR_MAXCTA = 160;  // flag columns per source rank (>= CTAs of one launch: 148)
+constexpr int DEC_AR_MAXCTA = 160;  // flag columns per source rank (>= CTAs of one launch: one per SM)
 int launch_decode1_allreduce(const MmArgs& a, const DecSets& sets, const DecodeAR& ar);  // b2q_decode.cu
 
-// Cluster barrier whose memory ordering is only CTA-scope: every cluster-scope release compiles to MEMBAR.ALL.GPU on
-// sm_100a (checked with cuobjdump), which waits on the whole memory system although the data exchanged here lives in
+// Cluster barrier whose memory ordering is only CTA-scope: a cluster-scope release can compile to MEMBAR.ALL.GPU,
+// which waits on the whole memory system although the data exchanged here lives in
 // shared memory, whose single point of coherence is the owning SM.  MEMBAR.ALL.CTA makes this thread's shared-memory
 // stores (and outstanding DSMEM loads) performed before the relaxed arrive.  Weaker than the PTX model asks for:
 // selected only with B2Q_DECODE2_FASTSYNC=1 (A/B switch), default is cluster_sync_all().
@@ -45,7 +45,7 @@ __device__ __forceinline__ uint32_t dec_ld_acquire_sys(const uint32_t* p) {
   return v;
 }
 
-// Row-parallel QuantLinear + all-reduce in ONE kernel (ar.world > 1; SURVEY.md §8e).  Every rank runs the same launch
+// Row-parallel QuantLinear + all-reduce in ONE kernel (ar.world > 1).  Every rank runs the same launch
 // plan on its K-shard, so CTA c of every rank finishes the same output rows.  Instead of storing them, the CTA
 //   1. pushes its fp32 partial sums into slot (seq & 1), row `rank`, of EVERY rank's symmetric buffer (P2P stores over
 //      NVLink; 128 B per warp and row),
@@ -473,7 +473,7 @@ static size_t decode2_smem(int M, int warps, int gw, int qpc, int max_tiles, int
 // Pick (split-K ranks, warps per CTA, warps per group) minimising the critical path in quads per warp.
 static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
   const int quads = a.K / 128;
-  const int SMS = 148;
+  const int SMS = num_sms();
   const int force_gw = env().decode2_gw;  // A/B switches (read once at load; b2q_debug_reload_env() re-reads them)
   const int force_ks = env().decode2_ks;
   double best_cost = 1e30;
@@ -503,7 +503,7 @@ static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
         if (smem > 200 * 1024) continue;
         const int qpw = (qpc + gw - 1) / gw;  // quads per warp per tile
         const double units = (double)max_tiles * qpw;
-        // main loop ~0.75 us per quad and warp at 16 warps / SM (profiles/r01_decode_notes.md); fewer warps hide less
+        // relative cost in units of one quad per warp at 16 warps / SM (heuristic weights); fewer warps hide less
         // latency; a tile switch costs a few dozen instructions; split-K adds a cluster barrier + DSMEM pass
         const double cost = units * (1.0 + (16 - warps) * 0.04) + 0.03 * max_tiles + (ks > 1 ? 0.5 : 0.0) +
                             0.02 * ngroups;

@@ -1,16 +1,16 @@
-// b2q_gemm.cu — prefill / batched path: out[M, N] = x[M, K] @ dequant(W)[K, N] (+ bias) on tcgen05 tensor cores.
+// b2q_gemm.cu — prefill / batched path: out[M, N] = x[M, K] @ dequant(W)[K, N] (+ bias) on Hopper wgmma tensor cores.
 //
-// One CTA computes a (128*MT tokens) x (128 features) output tile, K in blocks of 64, with a STAGES-deep
-// mbarrier ring and warp-specialised roles:
-//   warp 0      producer : TMA (cp.async.bulk.tensor, SWIZZLE_128B) for the activation tile and cp.async.bulk
-//                          for the packed int4/int8 weight tile (contiguous 2 KB B2Q rows), one elected lane
-//   warp 1      MMA      : allocates TMEM, one elected lane issues tcgen05.mma.cta_group::1.kind::f16
-//                          (M=128, N=128, K=16) with the fp32 accumulators in TMEM, tcgen05.commit -> mbarriers
-//   warps 2..5  dequant  : LDS.128 packed weights -> exact (q - z) * s in fp16/bf16 (integer subtract first, one
+// One CTA computes a 128 (tokens) x 128 (features) output tile, K in blocks of 64, with a STAGES-deep mbarrier ring and
+// warp-specialised roles:
+//   warps 0..3  MMA      : one warpgroup issues wgmma.mma_async m64n128k16 (two m64 blocks of tokens per k16 step), fp32
+//                          accumulators in registers; one wgmma group stays in flight, the stage of the block before it
+//                          is released to the producer; afterwards the same warps run the epilogue (+bias, fp16/bf16)
+//   warps 4..7  dequant  : LDS.128 packed weights -> exact (q - z) * s in fp16/bf16 (integer subtract first, one
 //                          rounding: identical operands to the reference's torch dequant, qlinear/__init__.py:
-//                          1001-1003) -> 16-byte swizzled K-major st.shared -> fence.proxy.async -> mbarrier;
-//                          afterwards the same warps run the epilogue: tcgen05.ld TMEM -> regs -> (+bias) ->
-//                          fp16/bf16 -> 64-byte-per-thread coalesced global stores.
+//                          1001-1003) -> 16-byte swizzled K-major st.shared -> fence.proxy.async -> mbarrier
+//   warp 8      producer : TMA (cp.async.bulk.tensor, SWIZZLE_128B) for the activation tile and cp.async.bulk
+//                          for the packed int4/int8 weight tile (contiguous B2Q rows), one elected lane
+// Sibling layers (q|k|v, gate|up) run in the same launch: blockIdx.x walks the tile columns of every weight set.
 // In the reference this is TorchLinear's dequant + torch.matmul (qlinear/torch.py:326-343), Marlin's
 // mma.sync kernel (marlin_template.h) and Swordfish's CUTLASS-derived prefill tier (swordfish_prefill_*.cuh).
 #include <cuda.h>
@@ -19,15 +19,15 @@
 #include "b2q_dequant.cuh"
 #include "b2q_gemm.cuh"
 #include "b2q_internal.h"
+#include "b2q_wgmma.cuh"
 
 namespace b2q {
 
-template <typename T, int BITS, bool ASYM, int MT, int STAGES>
+template <typename T, int BITS, bool ASYM, int STAGES>
 __global__ void __launch_bounds__(G_THREADS, 1)
-    gemm_kernel(const __grid_constant__ CUtensorMap tmap_x, const uint4* __restrict__ packed,
-                const T* __restrict__ scales, const uint32_t* __restrict__ qzeros, const T* __restrict__ bias,
-                T* __restrict__ out, int M, int K, int N, int group_size, int gshc) {
-  using C = GemmCfg<BITS, MT, STAGES>;
+    gemm_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ GemmSets S, int M, int K,
+                int gshc) {
+  using C = GemmCfg<BITS, STAGES>;
   using E = ET<T>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -38,36 +38,37 @@ __global__ void __launch_bounds__(G_THREADS, 1)
   const uint32_t sP = sB + STAGES * C::B_BYTES;
   const uint32_t sBar = sP + STAGES * C::P_BYTES;
   const uint32_t bar_full = sBar, bar_bready = sBar + 8 * STAGES, bar_empty = sBar + 16 * STAGES;
-  const uint32_t bar_tfull = sBar + 24 * STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + (sBar - smem_base) + 24 * STAGES + 8);
+
+  // weight set of this tile column
+  int set = 0, tn = blockIdx.x;
+  if (S.nsets > 1 && tn >= S.tn_end[0]) {
+    set = (S.nsets > 2 && tn >= S.tn_end[1]) ? 2 : 1;
+    tn -= S.tn_end[set - 1];
+  }
+  const int N = S.N[set];
+  const uint4* __restrict__ packed = S.packed[set];
+  const T* __restrict__ scales = reinterpret_cast<const T*>(S.scales[set]);
+  const uint32_t* __restrict__ qzeros = S.qzeros[set];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int NT = N >> 5;
-  const int n0 = blockIdx.x * G_BN, m0 = blockIdx.y * (128 * MT);
+  const int n0 = tn * G_BN, m0 = blockIdx.y * G_BM;
   const int nt0 = n0 >> 5;
   const int ntiles = min(4, NT - nt0);
   const int nkb = K / G_BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_bready + 8 * s, G_DQ_THREADS);
       mbar_init(bar_empty + 8 * s, 1);
     }
-    mbar_init(bar_tfull, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(tmem_ptr), C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================================ producer ================================
     if (lane == 0) {
       // 4-bit: the 128 x 64 tile is one contiguous block of T4 (8 feature tiles of 16); 8-bit: two T8 rows
@@ -81,13 +82,10 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         // 4-bit: scale / zero rows of the block's group(s) travel with the packed codes (no LDG in the dequant warps)
         const int g0 = (2 * kb) >> gshc, g1 = (2 * kb + 1) >> gshc;
         const int nrows = (g1 != g0) ? 2 : 1;
-        const uint32_t sbytes = (uint32_t)min(128, N - n0) * 2u, zbytes = ASYM ? sbytes / 4u : 0u;
+        const uint32_t sbytes = (uint32_t)min(G_BN, N - n0) * 2u, zbytes = ASYM ? sbytes / 4u : 0u;
         mbar_expect_tx(bar_full + 8 * s,
                        C::A_BYTES + (BITS == 4 ? pbytes4 + nrows * (sbytes + zbytes) : 2 * pbytes8));
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-          tma_load_2d(sA + s * C::A_BYTES + mt * (128 * G_BK * 2), &tmap_x, bar_full + 8 * s, kb * G_BK,
-                      m0 + mt * 128);
+        tma_load_2d(sA + s * C::A_BYTES, &tmap_x, bar_full + 8 * s, kb * G_BK, m0);
         if (BITS == 4) {
           bulk_load(sP + s * C::P_BYTES, packed + ((size_t)kb * FT + ft0) * 32, pbytes4, bar_full + 8 * s);
           for (int r = 0; r < nrows; ++r) {
@@ -105,33 +103,63 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ================================
-    constexpr uint32_t idesc = umma_idesc_f16(E::FMT, 128, G_BN);
+  } else if (warp < 4) {
+    // ================================ MMA warpgroup ================================
+    float acc[2][G_BN / 2];
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int i = 0; i < G_BN / 2; ++i) acc[mb][i] = 0.f;
     for (int kb = 0; kb < nkb; ++kb) {
       const int s = kb % STAGES;
       const uint32_t ph = (kb / STAGES) & 1;
       mbar_wait(bar_full + 8 * s, ph);
       mbar_wait(bar_bready + 8 * s, ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint64_t bdesc = umma_desc_k_sw128(sB + s * C::B_BYTES);
+      wgmma_fence();
+      const uint64_t bdesc = wgmma_desc_k_sw128(sB + s * C::B_BYTES);
+      const uint64_t adesc = wgmma_desc_k_sw128(sA + s * C::A_BYTES);
 #pragma unroll
-        for (int k = 0; k < G_BK / 16; ++k) {
+      for (int k = 0; k < G_BK / 16; ++k) {
 #pragma unroll
-          for (int mt = 0; mt < MT; ++mt) {
-            const uint64_t adesc = umma_desc_k_sw128(sA + s * C::A_BYTES + mt * (128 * G_BK * 2));
-            umma_f16(tbase + mt * G_BN, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(bar_empty + 8 * s);
-        if (kb == nkb - 1) umma_commit(bar_tfull);
+        for (int mb = 0; mb < 2; ++mb)
+          Wgmma<E::FMT, G_BN>::mma(acc[mb], adesc + 512 * mb + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
       }
-      __syncwarp();
+      wgmma_commit();
+      // the group of block kb - 1 has completed: its stage may be refilled
+      wgmma_wait<1>();
+      if (kb > 0 && threadIdx.x == 0) mbar_arrive(bar_empty + 8 * ((kb - 1) % STAGES));
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) wgmma_fence_regs(acc[mb]);
+
+    // ================================ epilogue ================================
+    const T* __restrict__ bias = reinterpret_cast<const T*>(S.bias[set]);
+    T* __restrict__ out = reinterpret_cast<T*>(S.out[set]);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = m0 + 64 * mb + 16 * warp + (lane >> 2) + 8 * h;
+        if (row >= M) continue;
+        T* dst = out + (size_t)row * N;
+#pragma unroll
+        for (int j = 0; j < G_BN / 8; ++j) {
+          const int col = n0 + 8 * j + 2 * (lane & 3);
+          if (col >= N) continue;
+          float f0 = acc[mb][4 * j + 2 * h], f1 = acc[mb][4 * j + 2 * h + 1];
+          if (bias != nullptr) {
+            // reference order: round the matmul to the output dtype, then add bias (torch.py:337-342)
+            f0 = E::to_f(E::from_f(f0)) + E::to_f(bias[col]);
+            f1 = E::to_f(E::from_f(f1)) + E::to_f(bias[col + 1]);
+          }
+          *reinterpret_cast<uint32_t*>(dst + col) = E::pack2(f0, f1);
+        }
+      }
     }
   } else {
-    // ================================ dequant warps ================================
-    const int t = threadIdx.x - 64;  // 0..127
+    // ================================ dequant warpgroup ================================
+    const int t = threadIdx.x - G_MMA_THREADS;  // 0..127
     constexpr int PF = 32 / BITS;
     constexpr int ZSYM = 1 << (BITS - 1);
     if (BITS == 4) {
@@ -225,46 +253,6 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         cur[1] = nxt[1];
       }
     }
-
-    // ================================ epilogue ================================
-    mbar_wait(bar_tfull, 0);
-    tc_fence_after();
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-      const int row = m0 + mt * 128 + q * 32 + lane;
-#pragma unroll
-      for (int cc = 0; cc < G_BN / 32; ++cc) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tbase + ((uint32_t)(q * 32) << 16) + mt * G_BN + cc * 32, r);
-        tmem_ld_wait();
-        const int nc = n0 + cc * 32;
-        if (row < M && nc < N) {
-          T* dst = out + (size_t)row * N + nc;
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              // reference order: round the matmul to the output dtype, then add bias (torch.py:337-342)
-              float f0 = __uint_as_float(r[v * 8 + 2 * i]), f1 = __uint_as_float(r[v * 8 + 2 * i + 1]);
-              if (bias != nullptr) {
-                f0 = E::to_f(E::from_f(f0)) + E::to_f(bias[nc + v * 8 + 2 * i]);
-                f1 = E::to_f(E::from_f(f1)) + E::to_f(bias[nc + v * 8 + 2 * i + 1]);
-              }
-              pk[i] = E::pack2(f0, f1);
-            }
-            *reinterpret_cast<uint4*>(dst + v * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-      }
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tbase, C::TMEM_COLS);
   }
 }
 
@@ -347,19 +335,60 @@ int gemm_gshc(const MmArgs& a) {
   return 31;
 }
 
-template <typename T, int BITS, bool ASYM, int MT, int STAGES>
-static int launch_gemm_t(const MmArgs& a, const void* x) {
-  using C = GemmCfg<BITS, MT, STAGES>;
+
+template <typename T, int BITS, bool ASYM, int STAGES>
+static int launch_gemm_t(const MmArgs& a, const void* x, const GemmSets& S) {
+  using C = GemmCfg<BITS, STAGES>;
   CUtensorMap tmap;
   if (make_x_tmap(&tmap, x, a.M, a.K, a.dtype) != 0) return -1;
-  auto kern = gemm_kernel<T, BITS, ASYM, MT, STAGES>;
+  auto kern = gemm_kernel<T, BITS, ASYM, STAGES>;
   static uint32_t smem_ok = 0;
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_ok, "b2q_gemm")) return e;
-  dim3 grid((a.N + G_BN - 1) / G_BN, (a.M + 128 * MT - 1) / (128 * MT), 1);
-  kern<<<grid, G_THREADS, C::SMEM_BYTES, a.stream>>>(tmap, (const uint4*)a.packed, (const T*)a.scales,
-                                                     (const uint32_t*)a.qzeros, (const T*)a.bias, (T*)a.out, a.M,
-                                                     a.K, a.N, a.group_size, gemm_gshc(a));
+  dim3 grid(S.tn_end[S.nsets - 1], (a.M + G_BM - 1) / G_BM, 1);
+  kern<<<grid, G_THREADS, C::SMEM_BYTES, a.stream>>>(tmap, S, a.M, a.K, gemm_gshc(a));
   return (int)cudaGetLastError();
+}
+
+static int launch_gemm_sets(const MmArgs& a, const void* x, const GemmSets& S) {
+  const bool asym = S.qzeros[0] != nullptr;
+#define B2Q_GEMM_CASE(T, BITS, ST) \
+  (asym ? launch_gemm_t<T, BITS, true, ST>(a, x, S) : launch_gemm_t<T, BITS, false, ST>(a, x, S))
+  if (a.dtype == 0) return a.bits == 4 ? B2Q_GEMM_CASE(__half, 4, 4) : B2Q_GEMM_CASE(__half, 8, 4);
+  return a.bits == 4 ? B2Q_GEMM_CASE(__nv_bfloat16, 4, 4) : B2Q_GEMM_CASE(__nv_bfloat16, 8, 4);
+#undef B2Q_GEMM_CASE
+}
+
+// Sibling QuantLinears in one launch (b2q_gemm_multi); x = activations with act-order already applied
+int launch_gemm_multi(const MmArgs& a, const void* x, int nsets, const void* const* packed, const void* const* scales,
+                      const int32_t* const* qzeros, const void* const* bias, void* const* out, const int* Ns) {
+  if (nsets < 1 || nsets > G_MAX_SETS) {
+    set_error("b2q_gemm_multi: nsets=%d out of range (1..%d)", nsets, G_MAX_SETS);
+    return -1;
+  }
+  if (a.K % G_BK != 0) {
+    set_error("b2q_gemm_multi: K=%d must be a multiple of %d", a.K, G_BK);
+    return -1;
+  }
+  GemmSets S = {};
+  S.nsets = nsets;
+  int tn = 0;
+  for (int i = 0; i < nsets; ++i) {
+    if (Ns[i] <= 0 || Ns[i] % 32 != 0 || packed[i] == nullptr || scales[i] == nullptr || out[i] == nullptr ||
+        ((qzeros[i] != nullptr) != (qzeros[0] != nullptr))) {
+      set_error("b2q_gemm_multi: set %d unsupported (N=%d; all sets share K, group size and symmetry)", i, Ns[i]);
+      return -1;
+    }
+    tn += (Ns[i] + G_BN - 1) / G_BN;
+    S.tn_end[i] = tn;
+    S.N[i] = Ns[i];
+    S.packed[i] = (const uint4*)packed[i];
+    S.scales[i] = scales[i];
+    S.qzeros[i] = (const uint32_t*)qzeros[i];
+    S.bias[i] = bias[i];
+    S.out[i] = out[i];
+  }
+  for (int i = nsets; i < G_MAX_SETS; ++i) S.tn_end[i] = tn;
+  return launch_gemm_sets(a, x, S);
 }
 
 int launch_gemm(const MmArgs& a) {
@@ -378,18 +407,14 @@ int launch_gemm(const MmArgs& a) {
     if (e != 0) return e;
     x = a.workspace;
   }
-  // M <= 128: small-batch tier (swapped operands, cluster split-K); B2Q_MIDM=0 keeps the round-1 padded single-CTA path
+  // M <= 128: small-batch tier (swapped operands, cluster split-K); B2Q_MIDM=0 keeps the padded 128-token tile
   if (a.M <= 128 && env().midm && midm_supported(a)) return launch_midm(a, x);
-  if (a.bits == 4 && a.M > 128 && a.tune_ks != -1)  // CTA-pair tier (tune_ks -1: force 1-CTA)
-    return launch_gemm2(a, x);
-  const bool asym = a.qzeros != nullptr;
-  const bool big = a.M > 128;
-#define B2Q_GEMM_CASE(T, BITS, ST)                                                              \
-  (asym ? (big ? launch_gemm_t<T, BITS, true, 2, ST>(a, x) : launch_gemm_t<T, BITS, true, 1, ST>(a, x)) \
-        : (big ? launch_gemm_t<T, BITS, false, 2, ST>(a, x) : launch_gemm_t<T, BITS, false, 1, ST>(a, x)))
-  if (a.dtype == 0) return a.bits == 4 ? B2Q_GEMM_CASE(__half, 4, 4) : B2Q_GEMM_CASE(__half, 8, 3);
-  return a.bits == 4 ? B2Q_GEMM_CASE(__nv_bfloat16, 4, 4) : B2Q_GEMM_CASE(__nv_bfloat16, 8, 3);
-#undef B2Q_GEMM_CASE
+  const void* packed = a.packed;
+  const void* scales = a.scales;
+  const int32_t* qzeros = (const int32_t*)a.qzeros;
+  const void* bias = a.bias;
+  void* out = a.out;
+  return launch_gemm_multi(a, x, 1, &packed, &scales, &qzeros, &bias, &out, &a.N);
 }
 
 }  // namespace b2q

@@ -1,13 +1,13 @@
 // b2q_gemv.cu — 8-bit, batch-1 decode path: out[n] = sum_k x[k] * s[g(k), n] * (q[k, n] - z[g(k), n])  (+ bias).
 //
 // CUDA-core tier on the T8 layout (uint4 T8[K/32][N/32][2][32], natural byte order).  (The 4-bit decode path started
-// as this kernel, was found issue-bound — profiles/r01_gemv_r1a.txt — and moved to b2q_decode.cu.)
+// as this kernel, is issue-bound and lives in b2q_decode.cu on mma.sync.)
 //  * grid = (N/32 feature tiles) x (KS split-K CTAs); the KS CTAs of one feature tile form a thread-block cluster
 //    and reduce their partial sums through distributed shared memory (no atomics, no workspace, deterministic);
 //  * each lane owns ONE output feature; a warp reads 32 features x 16 k per coalesced 512-byte request, 8 requests in
 //    flight per lane, issued BEFORE griddepcontrol.wait / the activation staging (weights do not depend on x);
-//  * PRMT builds exact 1024+q half pairs; the multiply-accumulate is the sm_100a mixed-precision FMA
-//    fma.rn.f32.f16 (SASS FHFMA): exact fp16 x fp16 product, fp32 accumulate.  The zero-point and the 1024 bias
+//  * PRMT builds exact 1024+q half pairs; the multiply-accumulate is an fp32 FMA of the exactly widened halves:
+//    exact fp16 x fp16 product, fp32 accumulate.  The zero-point and the 1024 bias
 //    are removed once per group with pre-reduced activation sums: sum (q-z) x = sum (1024+q) x - (1024+z) sum x;
 //  * act-order: rows sorted by group at prepack; the x[perm[k']] gather is fused into the smem staging.
 // Replaces, for 8-bit M == 1, TorchLinear.forward (qlinear/torch.py:302-347) / Marlin's small-M path.
@@ -265,7 +265,7 @@ static void gemv_config(const MmArgs& a, int& ks, int& warps, int& cpc) {
     ks = a.tune_ks;
   } else {
     ks = 1;
-    while (ks < 8 && NT * ks < 148 * 6 && quads / (ks * 2) >= 1) ks *= 2;
+    while (ks < 8 && NT * ks < num_sms() * 6 && quads / (ks * 2) >= 1) ks *= 2;
   }
   while (4 * ((quads + ks - 1) / ks) > GEMV_MAX_CPC && ks < 16) ks *= 2;
   cpc = 4 * ((quads + ks - 1) / ks);

@@ -1,48 +1,48 @@
 // b2q_midm.cu — small-batch tier (2 <= tokens <= 128; every 8-bit / group_size 32 shape the decode tier does not
-// take): out[M, N] = x[M, K] @ dequant(W)[K, N] (+ bias) with SWAPPED tcgen05 operands and cluster split-K.
+// take): out[M, N] = x[M, K] @ dequant(W)[K, N] (+ bias) with SWAPPED wgmma operands and cluster split-K.
 //
 // Batched decode / speculative decoding is HBM-bound like batch-1 decode: the layer's packed weights must stream once,
-// the token count only changes the width of the MMA.  The prefill tiers pad tokens to the UMMA M = 128 and launch
-// N/128 CTAs (32 of 148 SMs for a 4096-wide layer: 28 us for 4096 x 4096 at any M <= 128, 0.05 of the HBM roofline —
-// VERDICT r01 weak #4).  Here
-//   * the WEIGHTS are the UMMA A operand: 128 output features = the M = 128 rows of tcgen05.mma.cta_group::1.kind::f16,
-//     the TOKENS are the B operand, N = NTOK in {16, 32, 64, 128}: no padding of tokens to 128, the accumulator
-//     D[feature][token] needs only NTOK TMEM columns and the x tile is NTOK x 64 k (TMA, SWIZZLE_128B);
+// the token count only changes the width of the MMA.  The prefill tier pads tokens to its 128-token tile and launches
+// N/128 CTAs (32 of 132 SMs for a 4096-wide layer).  Here
+//   * the WEIGHTS are the wgmma A operand: 128 output features = two m64 blocks, the TOKENS are the B operand,
+//     N = NTOK in {16, 32, 64, 128}: no padding of tokens to 128, the accumulator D[feature][token] is NTOK registers per
+//     thread of the MMA warpgroup and the x tile is NTOK x 64 k (TMA, SWIZZLE_128B);
 //   * `ks` CTAs of a thread-block cluster split the k-blocks of one 128-feature tile (4096 x 4096: 32 tiles x 4 = 128
 //     CTAs), park their fp32 partials TRANSPOSED ([token][feature]) in their own shared memory and reduce an interleaved
 //     share of the token rows over distributed shared memory: no atomics, no workspace, deterministic, and the global
 //     stores are 256 contiguous bytes per warp (features are the fast axis of `out`);
-//   * 8 dequant warps (one fragment-major uint4 = 2 features x 16 k per thread and k-block) produce the exact
-//     (q - z) * s operand (integer subtract first, ONE rounding: qlinear/__init__.py:1001-1003) as 16-byte swizzled
-//     K-major rows.  The dequant warps form 4 groups that take every 4th k-block; each group's leader issues the bulk copies of
-//     the group's own packed stages, warp 0 only the x tile TMA: no single thread issues every asynchronous copy of every
-//     k-block, and the weight stream + dequant of the first blocks run BEFORE griddepcontrol.wait (programmatic dependent
-//     launch), i.e. under the previous kernel's tail.
+//   * 4 dequant warps (fragment-major uint4 = 2 features x 16 k each) produce the exact (q - z) * s operand (integer
+//     subtract first, ONE rounding: qlinear/__init__.py:1001-1003) as 16-byte swizzled K-major rows.  Each dequant warp
+//     takes every 4th k-block and issues the bulk copies of its own packed stages, warp 8 only the x tile TMA: no single
+//     thread issues every asynchronous copy of every k-block, and the weight stream + dequant of the first blocks run
+//     BEFORE griddepcontrol.wait (programmatic dependent launch), i.e. under the previous kernel's tail.
 // Reference counterparts: Swordfish's Stream-K / atomic split-K decode for 17 <= M < 128 (swordfish_mm.cu:113-154,
-// 229-276), its swapped-problem-shape tcgen05 trick (swordfish_prefill_impl.cuh:219-227), Marlin's small-M tiles
+// 229-276), its swapped-problem-shape trick (swordfish_prefill_impl.cuh:219-227), Marlin's small-M tiles
 // (marlin_template.h).
 #include <cuda.h>
 
 #include "b2q_common.cuh"
 #include "b2q_dequant.cuh"
 #include "b2q_internal.h"
+#include "b2q_wgmma.cuh"
 
 namespace b2q {
 
-constexpr int MM_BF = 128;                  // features per tile (UMMA M)
+constexpr int MM_BF = 128;                  // features per tile (two wgmma m64 blocks)
 constexpr int MM_BK = 64;                   // k per block (one SWIZZLE_128B row of fp16)
-constexpr int MM_DQ_WARPS = 8;
+constexpr int MM_MMA_THREADS = 128;         // warps 0..3: the wgmma warpgroup
+constexpr int MM_DQ_WARPS = 4;              // warps 4..7
 constexpr int MM_DQ_THREADS = MM_DQ_WARPS * 32;
-constexpr int MM_THREADS = 64 + MM_DQ_THREADS + 96;  // producer, MMA issuer 0, 8 dequant warps, MMA issuers 1..3 (warps 10..12)
+constexpr int MM_THREADS = MM_MMA_THREADS + MM_DQ_THREADS + 32;  // + warp 8: activation producer
+constexpr int MM_RED_WARPS = 8;             // warps 0..7 reduce the split-K partials
 
 // Two rings.  The PACKED ring (PST stages: x tile + packed codes + scale / zero rows, 7-21 KB each) is what hides the HBM
 // latency: with 4 stages (the first version of this kernel) only 16 KB of weights per SM were in flight and every k-block
-// cost ~0.39 us = one HBM round trip / 4 (profiles/r02_midm_v1_bench.log: 25 us for the 64 k-blocks of 4096 x 4096 on one
-// CTA per tile); Little's law asks for ~43 KB per SM at 6.5 TB/s.  The DEQUANTISED ring (WST stages of 16 KB) only
+// cost one HBM round trip / 4; Little's law asks for tens of KB in flight per SM.  The DEQUANTISED ring (WST stages of 16 KB) only
 // decouples the dequant warps from the tensor core.
 // MODE 0: one QuantLinear.  MODE 1 / 2: GROUPED over the experts of a MoE block (b2q_moe.cu): blockIdx.z = (expert, token
 // block); the rows of an expert are contiguous in the expert-sorted activation matrix; CTAs beyond an expert's row count
-// exit at once.  MODE 1 runs TWO weight sets (w1 = gate, w3 = up) through the pipeline back to back into two TMEM
+// exit at once.  MODE 1 runs TWO weight sets (w1 = gate, w3 = up) through the pipeline back to back into two register
 // accumulators and stores silu(gate) * up; MODE 2 (w2 = down) scales each row by its routing weight and scatters it to the
 // row's (token, k) slot of an fp32 buffer.
 struct MoeArgs {
@@ -69,26 +69,15 @@ struct MidCfg {
   static constexpr int BAR_BYTES = 512;
   static constexpr int RING_BYTES = WST * W_BYTES + XST * X_BYTES + PST * P_BYTES;
   static constexpr int SMEM_BYTES = RING_BYTES + BAR_BYTES + 1024;
-  static constexpr int ACC_COLS = NSETS * NTOK;          // one accumulator set per MMA issuer
-  static constexpr int NISS = 4 * ACC_COLS <= 512 ? 4 : 2;  // MMA issuer warps (k-blocks i, i + NISS, ... each)
-  static constexpr int TMEM_COLS = NISS * ACC_COLS < 32 ? 32 : NISS * ACC_COLS;
-  static_assert(XST % NISS == 0 && WST % NISS == 0, "every use of a stage must belong to the same MMA issuer");
+  static constexpr int ACC = NTOK / 2;                   // fp32 accumulator registers per thread, per set and m64 block
+  static_assert(NSETS * NTOK <= 128, "accumulators of the MMA warpgroup: at most 128 registers per thread");
   static constexpr int PART_BYTES = NSETS * NTOK * MM_BF * 4;  // fp32 partial tile(s) [set][token][feature]
   static_assert(MODE == 0 || BITS == 4, "the grouped (MoE) modes are built for 4-bit experts");
   static_assert(X_BYTES % 1024 == 0, "x tiles must stay 1024-byte aligned (SWIZZLE_128B atoms)");
   static_assert(PART_BYTES <= RING_BYTES, "the fp32 partial tile reuses the idle stage buffers");
-  static_assert((PST + 2 * XST + 2 * WST + 1) * 8 + 16 <= BAR_BYTES, "mbarrier area");
+  static_assert((PST + 2 * XST + 2 * WST) * 8 <= BAR_BYTES, "mbarrier area");
   static_assert(SMEM_BYTES <= 227 * 1024, "dynamic shared memory of one CTA");
 };
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
 
 template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE, int DQG>
 __global__ void __launch_bounds__(MM_THREADS, 1)
@@ -132,8 +121,7 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
   const uint32_t sPr = sXr + XST * C::X_BYTES;        // [PST]{ packed codes | scale / zero rows }
   const uint32_t sBar = sPr + PST * C::P_BYTES;
   const uint32_t bar_pfull = sBar, bar_xfull = bar_pfull + 8 * PST, bar_xempty = bar_xfull + 8 * XST;
-  const uint32_t bar_wready = bar_xempty + 8 * XST, bar_wempty = bar_wready + 8 * WST, bar_tfull = bar_wempty + 8 * WST;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + (bar_tfull - smem_base) + 8);
+  const uint32_t bar_wready = bar_xempty + 8 * XST, bar_wempty = bar_wready + 8 * WST;
   auto sXs = [&](int s) { return sXr + (uint32_t)s * C::X_BYTES; };
   auto sPs = [&](int s) { return sPr + (uint32_t)s * C::P_BYTES; };
 
@@ -151,7 +139,7 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
   // PDL: the next kernel in the stream may start its own prologue / weight prefetch now
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_x);
     for (int s = 0; s < PST; ++s) mbar_init(bar_pfull + 8 * s, 1);
     for (int s = 0; s < XST; ++s) {
@@ -162,21 +150,13 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
       mbar_init(bar_wready + 8 * s, MM_DQ_THREADS / DQG);
       mbar_init(bar_wempty + 8 * s, 1);
     }
-    mbar_init(bar_tfull, nkb >= C::NISS ? C::NISS : (nkb >= 2 ? 2 : 1));  // one arrival per active MMA issuer
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(tmem_ptr), C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tbase = *tmem_ptr;
 
   // ---- weight loads of pipeline iteration i into packed stage s (issued by the LEADER of the dequant group that will
-  // consume the stage, see below: one thread per SM issuing every asynchronous copy of every k-block was the k-block time,
-  // ~150 clk per UBLKCP / UTMALDG from a single thread — profiles/r02_midm_notes.md)
+  // consume the stage, see below: one thread per SM issuing every asynchronous copy of every k-block serialises the
+  // copy issue)
   const int FT = N >> 4, ft0 = n0 >> 4;
   const uint32_t pbytes4 = (uint32_t)min(8, FT - ft0) * 512u;
   const uint32_t pbytes8 = (uint32_t)ntiles * C::SUB * 512u;
@@ -208,7 +188,7 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
     }
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================================ activation producer ================================
     // one TMA per pipeline iteration: the x tile of the k-block (the weights are loaded by the dequant group leaders)
     if (lane == 0) {
@@ -221,48 +201,73 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
         tma_load_2d(sXs(xs), &tmap_x, bar_xfull + 8 * xs, kb * MM_BK, row0);
       }
     }
-  } else if (warp == 1 || warp >= 10) {
-    // ================================ MMA issuers ================================
-    // Up to FOUR issuing warps take every NISS-th pipeline iteration and accumulate into their OWN TMEM columns (summed in
-    // the epilogue: deterministic).  One thread issuing the two mbarrier waits, four tcgen05.mma and two or three
-    // tcgen05.commit of EVERY k-block was the k-block time of this tier (~770 clk at any token width, ring depth, dequant
-    // parallelism or copy-issue scheme: profiles/r02_midm_notes.md).
-    constexpr uint32_t idesc = umma_idesc_f16(E::FMT, MM_BF, NTOK);
-    const int nissue = nkb >= C::NISS ? C::NISS : (nkb >= 2 ? 2 : 1);
-    const int mi = warp == 1 ? 0 : warp - 9;
-    for (int i = mi; i < NI && mi < nissue; i += nissue) {
+  } else if (warp < 4) {
+    // ================================ MMA warpgroup ================================
+    // One wgmma group (4 k16 steps x 2 m64 feature blocks) per pipeline iteration, one group kept in flight: the stages of
+    // iteration i - 1 are released once the group of iteration i has been issued and i - 1 has completed.
+    float acc[NSETS][2][C::ACC];
+#pragma unroll
+    for (int st = 0; st < NSETS; ++st)
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int v = 0; v < C::ACC; ++v) acc[st][mb][v] = 0.f;
+    // one loop per weight set: the wgmma of a loop always targets the same accumulator registers (a set chosen at run time
+    // inside the loop would put the wgmma on a divergent path, which ptxas serialises)
+    auto step = [&](int i, float (&ac)[2][C::ACC], bool first) {
       const int xs = i % XST, ws = i % WST;
       mbar_wait(bar_xfull + 8 * xs, (i / XST) & 1);
       mbar_wait(bar_wready + 8 * ws, (i / WST) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const bool second = NSETS > 1 && i >= nkb;
-        // accumulator of (issuer mi, set): TMEM columns (mi * NSETS + set) * NTOK
-        const uint32_t dcol = tbase + (uint32_t)(mi * C::ACC_COLS + (second ? NTOK : 0));
-        const int start = second ? nkb : 0;
-        const int first = start + ((mi - start % nissue + nissue) % nissue);  // this issuer's first block of the set
-        const uint64_t wdesc = umma_desc_k_sw128(sW + ws * C::W_BYTES);
-        const uint64_t xdesc = umma_desc_k_sw128(sXs(xs));
+      // wready(i) completed => the dequant group has read packed stage i % PST: stream block i + PST into it (one
+      // thread per k-block, off the dequant groups' latency chain)
+      if (ISSUER_REFILL && threadIdx.x == 0 && i + PST < NI) load_weights(i + PST, i % PST);
+      const uint64_t wdesc = wgmma_desc_k_sw128(sW + ws * C::W_BYTES);
+      const uint64_t xdesc = wgmma_desc_k_sw128(sXs(xs));
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < MM_BK / 16; ++k)
-          umma_f16(dcol, wdesc + 2 * k, xdesc + 2 * k, idesc, (i != first || k != 0) ? 1u : 0u);
-        umma_commit(bar_wempty + 8 * ws);  // the dequantised stage may be overwritten
-        umma_commit(bar_xempty + 8 * xs);  // the x tile has been read
-        if (i + nissue >= NI) umma_commit(bar_tfull);  // this issuer's last block
-        // wready(i) completed => the dequant group has read packed stage i % PST: stream block i + PST into it (one
-        // issuer thread per k-block class, off the dequant groups' latency chain)
-        if (ISSUER_REFILL && i + PST < NI) load_weights(i + PST, i % PST);
+      for (int k = 0; k < MM_BK / 16; ++k) {
+#pragma unroll
+        for (int mb = 0; mb < 2; ++mb)  // the first block of a set overwrites
+          Wgmma<E::FMT, NTOK>::mma(ac[mb], wdesc + 512 * mb + 2 * k, xdesc + 2 * k, (first && k == 0) ? 0u : 1u);
       }
-      __syncwarp();
-    }
-  } else if (warp < 10) {
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (i > 0 && threadIdx.x == 0) {
+        mbar_arrive(bar_wempty + 8 * ((i - 1) % WST));  // the dequantised stage may be overwritten
+        mbar_arrive(bar_xempty + 8 * ((i - 1) % XST));  // the x tile has been read
+      }
+    };
+    for (int i = 0; i < nkb; ++i) step(i, acc[0], i == 0);
+    if (NSETS > 1)
+      for (int i = nkb; i < NI; ++i) step(i, acc[NSETS - 1], i == nkb);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int st = 0; st < NSETS; ++st)
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) wgmma_fence_regs(acc[st][mb]);
+
+    // ---- this rank's fp32 accumulator D[feature][token] -> its own shared memory, transposed: part[set][token][feature]
+    // (the stage buffers are idle now: every load was consumed by an MMA that has completed)
+#pragma unroll
+    for (int st = 0; st < NSETS; ++st)
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int v = 0; v < C::ACC; ++v) {
+          const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
+          const int feat = 64 * mb + 16 * warp + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(sW + (uint32_t)((st * NTOK + tok) * MM_BF + feat) * 4),
+                       "f"(acc[st][mb][v])
+                       : "memory");
+        }
+  } else {
     // ================================ dequant warps ================================
     // The dequant warps form DQG groups of TG threads; group gq takes the pipeline iterations i = gq, gq + DQG, ...  One
     // iteration is a serial chain of latencies for a warp (mbarrier wake-up, LDS, ~75 ALU instructions per uint4, STS,
     // fence.proxy.async, arrive: ~800 clk) — with all eight warps on the SAME k-block (first version) that chain WAS the
-    // k-block time (0.43 us per k-block at any ring depth, profiles/r02_midm_notes.md); with DQG blocks in flight the
+    // k-block time at any ring depth; with DQG blocks in flight the
     // chains overlap and the tier becomes issue-bound instead.
-    const int t = threadIdx.x - 64;  // 0..255
+    const int t = threadIdx.x - MM_MMA_THREADS;  // 0..127
     constexpr int TG = MM_DQ_THREADS / DQG;
     static_assert(PST % DQG == 0 && WST % DQG == 0, "every use of a ring stage must belong to the same dequant group");
     const int gq = t / TG, tl = t - gq * TG;
@@ -273,8 +278,8 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
     if (tl == 0)
       for (int i = gq; i < NI && i < PST; i += DQG) load_weights(i, i);
     if (BITS == 4) {
-      // DQG fragment-major uint4 per thread and iteration: q = tl + TG*u -> feature tile q>>5 (16 features), lane' = q&31
-      constexpr int U = DQG;
+      // U fragment-major uint4 per thread and iteration: q = tl + TG*u -> feature tile q>>5 (16 features), lane' = q&31
+      constexpr int U = 256 / TG;
       const int lp = tl & 31, g = lp >> 2, tt = lp & 3;
       for (int i = gq; i < NI; i += DQG) {
         const int kb = kb0 + ((NSETS > 1 && i >= nkb) ? i - nkb : i), s = i % PST, ws = i % WST;
@@ -303,8 +308,8 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
         }
         // Refill of the packed stage for block i + PST.  With >= 3 packed stages per group the MMA issuer of block i does it
         // (it observes wready(i), which this group only signals after every thread has read the stage: no barrier or copy
-        // issue inside this chain; 7.7 -> 7.5 us at M = 16).  With 1-2 stages per group that is too late — the group would
-        // wait a full HBM round trip per block (M = 128: 10.7 -> 12.3 us measured) — so the group's leader refills right
+        // issue inside this chain).  With 1-2 stages per group that is too late — the group would
+        // wait a full HBM round trip per block — so the group's leader refills right
         // after the whole group has read.
         if (!ISSUER_REFILL) {
           asm volatile("bar.sync %0, %1;" ::"r"(1 + gq), "r"(TG) : "memory");
@@ -392,47 +397,19 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
         mbar_arrive(bar_wready + 8 * ws);
       }
     }
-
-    // ---- this rank's fp32 accumulator D[feature][token] -> its own shared memory, transposed: part[token][feature]
-    // (the stage buffers are idle once bar_tfull fired: every load was consumed by an MMA that has completed)
-    mbar_wait(bar_tfull, 0);
-    tc_fence_after();
-    asm volatile("griddepcontrol.wait;" ::: "memory");  // (already satisfied) orders the global stores below
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;       // two warps share a quarter: they split the 16-token column chunks
-    // column chunk c of 16 tokens; with two weight sets the chunks NTOK/16 .. 2*NTOK/16-1 are set 1 (TMEM columns and
-    // partial-tile rows continue seamlessly: part[set * NTOK + token][feature])
-    const int nacc = nkb >= C::NISS ? C::NISS : (nkb >= 2 ? 2 : 1);  // accumulators in use (one per active MMA issuer)
-    for (int c = half; c < NSETS * NTOK / 16; c += 2) {
-      uint32_t r[16];
-      tmem_ld_32x32b_x16(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 16), r);
-      tmem_ld_wait();
-      for (int ai = 1; ai < nacc; ++ai) {  // fixed order: deterministic
-        uint32_t r2[16];
-        tmem_ld_32x32b_x16(tbase + ((uint32_t)(q * 32) << 16) + (uint32_t)(ai * C::ACC_COLS + c * 16), r2);
-        tmem_ld_wait();
-#pragma unroll
-        for (int v = 0; v < 16; ++v) r[v] = __float_as_uint(__uint_as_float(r[v]) + __uint_as_float(r2[v]));
-      }
-#pragma unroll
-      for (int v = 0; v < 16; ++v)
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW + (uint32_t)(c * 16 + v) * (MM_BF * 4) + (uint32_t)(q * 32 + lane) * 4),
-                     "r"(r[v])
-                     : "memory");
-    }
-    tc_fence_before();
   }
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // (already satisfied) orders the global stores below
   // all ranks' partials are in place (cluster barrier = CTA barrier + cross-CTA release / acquire)
   __syncwarp();
   cluster_sync_all();
-  if (warp >= 2 && warp < 10) {
+  if (warp < MM_RED_WARPS) {
     // rank z reduces token rows z, z + nrank, ... over all ranks through distributed shared memory; a warp owns one
     // token row at a time: 32 lanes x 4 features = the 128 features of the tile = 256 contiguous output bytes
-    const int t = threadIdx.x - 64;
+    const int t = threadIdx.x;
     const int chunk = t & 31;
     const int nc = n0 + chunk * 4;
     if (nc < N) {
-      for (int tok = (int)crank + (int)nrank * (t >> 5); tok < M; tok += (int)nrank * MM_DQ_WARPS) {
+      for (int tok = (int)crank + (int)nrank * (t >> 5); tok < M; tok += (int)nrank * MM_RED_WARPS) {
         const uint32_t local = sW + (uint32_t)tok * (MM_BF * 4) + (uint32_t)chunk * 16;
         float acc[4] = {0.f, 0.f, 0.f, 0.f}, acc2[4] = {0.f, 0.f, 0.f, 0.f};
         for (uint32_t r = 0; r < nrank; ++r) {
@@ -495,10 +472,6 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tbase, C::TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -506,11 +479,11 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 int make_x_tmap_box(CUtensorMap* map, const void* x, int M, int K, int dtype, int box_rows);  // b2q_gemm.cu
 
-// split-K ranks (cluster size) for one launch: fill ~148 SMs, keep >= 4 k-blocks per rank, portable cluster size <= 8
+// split-K ranks (cluster size) for one launch: fill the SMs, keep >= 4 k-blocks per rank, portable cluster size <= 8
 int midm_ranks(int K, int N) {
   const int tiles = (N + MM_BF - 1) / MM_BF, nkb = K / MM_BK;
   int ks = 1;
-  while (ks < 8 && tiles * ks * 2 <= 148 && nkb / (ks * 2) >= 4) ks *= 2;
+  while (ks < 8 && tiles * ks * 2 <= num_sms() && nkb / (ks * 2) >= 4) ks *= 2;
   return ks;
 }
 
@@ -564,7 +537,7 @@ int launch_midm(const MmArgs& a, const void* x) {
   // consecutive uses of a stage belonged to different groups, a group that ran two uses ahead saw the phase of use u - 2 as
   // "its" completed phase, consumed a stage that had not been refilled and corrupted the arrival counts — every
   // single-launch parity test and all three sanitizer tools passed, back-to-back launches at full size faulted
-  // (profiles/r02_midm_notes.md).  8 dequantised stages = two per group; 4-8 packed stages (refilled by the group's own
+  // .  8 dequantised stages = two per group; 4-8 packed stages (refilled by the group's own
   // leader); 4-8 activation stages in their own ring.
 #define B2Q_MM_NTOK(T, BITS, AS)                                                                  \
   (a.M <= 16   ? launch_midm_t<T, BITS, AS, 16, (BITS == 4 ? 12 : 8), 8>(a, x, ks)                \
@@ -586,7 +559,7 @@ int launch_midm(const MmArgs& a, const void* x) {
 int midm_grouped_ranks(int K, int N, int active) {
   const int tiles = (N + MM_BF - 1) / MM_BF, nkb = K / MM_BK;
   int ks = 1;
-  while (ks < 8 && tiles * active * ks * 2 <= 148 && nkb / (ks * 2) >= 4) ks *= 2;
+  while (ks < 8 && tiles * active * ks * 2 <= num_sms() && nkb / (ks * 2) >= 4) ks *= 2;
   return ks;
 }
 
@@ -607,7 +580,8 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   G.ypair = g.ypair;
   // token-box width: every expert may receive up to `rows` rows; boxes of 16 serve decode-sized batches with one block
   // per expert, larger batches take 128-row blocks (CTAs of blocks beyond an expert's count exit immediately)
-  const int ntok = g.rows <= 16 ? 16 : g.rows <= 32 ? 32 : g.rows <= 64 ? 64 : 128;
+  // (mode 1 holds two accumulator sets in the registers of the MMA warpgroup: blocks of at most 64 tokens)
+  const int ntok = g.rows <= 16 ? 16 : g.rows <= 32 ? 32 : (g.rows <= 64 || mode == 1) ? 64 : 128;
   G.tblocks = (g.rows + ntok - 1) / ntok;
   const int grid_z = g.E * G.tblocks;
   int ks = env().midm_ks > 0 ? env().midm_ks : midm_grouped_ranks(a.K, a.N, g.active > 0 ? g.active : 1);
@@ -619,7 +593,7 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   (ntok == 16   ? launch_midm_t<T, 4, AS, 16, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
    : ntok == 32 ? launch_midm_t<T, 4, AS, 32, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
    : ntok == 64 ? launch_midm_t<T, 4, AS, 64, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
-                : launch_midm_t<T, 4, AS, 128, 4, 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
+                : launch_midm_t<T, 4, AS, (MODE == 1 ? 64 : 128), (MODE == 1 ? 8 : 4), 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
 #define B2Q_MG_CASE(T)                                                                       \
   (mode == 1 ? (asym ? B2Q_MG_NTOK(T, true, 1) : B2Q_MG_NTOK(T, false, 1))                   \
              : (asym ? B2Q_MG_NTOK(T, true, 2) : B2Q_MG_NTOK(T, false, 2)))

@@ -1,4 +1,4 @@
-// b2q_moe.cu — routing helpers of the grouped MoE expert path (BASELINE configs[4]: Mixtral-8x7B int4 g64 asym; SURVEY §8e).
+// b2q_moe.cu — routing helpers of the grouped MoE expert path (BASELINE configs[4]: Mixtral-8x7B int4 g64 asym).
 //
 // The reference ships a fused MoE op it never calls (swordfish_moe.cu:9-17,38-48: moe_align_block_size(16) ->
 // sorted_token_ids / expert_ids -> one grouped launch); its models run every expert's w1 / w3 / w2 QuantLinear from a Python

@@ -87,8 +87,7 @@ int launch_prepack(const void* qweight, const int32_t* perm, void* out, int K, i
 
 // x'[m, k'] = x[m, perm[k']]  (act-order activation gather for the tensor-core tiers; the decode tiers fuse it).
 // Same job as permute_cols_kernel in the reference's Marlin (gptq_marlin.cu:86-164).
-// Round 2 issued one 2-byte global load per element (M x K uncoalesced requests: the act-order prefill ran at 922 instead of
-// 1089 TFLOP/s).  Here a CTA stages one row of x in shared memory with coalesced 16-byte loads, gathers from shared memory
+// One 2-byte global load per element would be M x K uncoalesced requests.  Here a CTA stages one row of x in shared memory with coalesced 16-byte loads, gathers from shared memory
 // and writes 16-byte rows; the thread's slice of `perm` is read once and reused for every row the CTA walks.
 template <int UNITS>
 __global__ void __launch_bounds__(256)
@@ -146,7 +145,7 @@ static int launch_permute_rows(const void* x, const int32_t* perm, void* out, in
   auto kern = permute_rows_kernel<UNITS>;
   const size_t smem = (size_t)K * 2;  // <= 32 KB: inside the default dynamic shared memory limit
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(M < 148 * 8 ? M : 148 * 8, 1, 1);
+  cfg.gridDim = dim3(M < num_sms() * 8 ? M : num_sms() * 8, 1, 1);
   cfg.blockDim = dim3(256, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;

@@ -1,7 +1,7 @@
 """Checkpoint bit layouts the kernels do not read natively, and their exact conversion into the ones they do.
 
 The B200 kernels stream 4- and 8-bit codes.  The reference's GPTQ QuantLinear contract is wider
-(/root/reference/gptqmodel/nn_modules/qlinear/__init__.py:766-785, :907-999; utils/planar_packing.py:1-52):
+(gptqmodel/nn_modules/qlinear/__init__.py:766-785, :907-999; utils/planar_packing.py:1-52):
 
   * 2-bit                      16 codes per int32 word, LSB first (same scheme as 4 / 8-bit),
   * 3-bit "continuous"         32 codes = one 96-bit little-endian bit stream over 3 consecutive words
@@ -14,7 +14,7 @@ A b-bit code with a b-bit zero-point is the same integer in a wider container, a
 container: `widen()` re-packs such a layer into the 4-bit (b <= 4) or 8-bit (b >= 5) LSB-first layout, bit-exactly, once,
 at `post_init()` time, on the device the checkpoint tensors live on (torch integer ops: load-time plumbing, not the hot
 path).  The price is memory and bandwidth (a 2-bit layer streams 4 bits per weight, a 5-bit layer 8): the arithmetic is
-the reference's, the footprint is the container's.  DESIGN.md §6 states this trade-off.
+the reference's, the footprint is the container's.
 
 `regroup()` handles an ARBITRARY g_idx (groups of unequal size, e.g. a K-slice of an act-order layer whose scale table
 is replicated across tensor-parallel ranks, utils/marlin.py:296-305): rows are sorted by group, every group's run is padded

@@ -1,8 +1,8 @@
-"""Checkpoint loader for real GPTQ / AWQ safetensors checkpoints (SURVEY.md §8 row f2).
+"""Checkpoint loader for real GPTQ / AWQ safetensors checkpoints.
 
 What the reference does for this step, restated for this package (no model definitions, no accelerate):
   * the quantisation config is read from ``quantize_config.json``, ``quant_config.json`` or the ``quantization_config``
-    entry of ``config.json``, in that order (/root/reference/gptqmodel/quantization/config.py:73-74), with the legacy
+    entry of ``config.json``, in that order (gptqmodel/quantization/config.py:73-74), with the legacy
     aliases ``w_bit / wbits -> bits``, ``q_group_size -> group_size``, ``version / checkpoint_format -> format``,
     ``quant_method -> method`` and ``zero_point -> not sym`` (config.py:1504-1525);
   * ``dynamic`` maps module-name regexes to per-module overrides; the FIRST matching pattern wins, a ``-:`` prefix means

@@ -1,10 +1,10 @@
-"""Fused neighbours of the GEMM (SURVEY.md §8 row f1): ``act_fn(gate_proj(x)) * up_proj(x)`` of a Llama-style MLP in ONE
+"""Fused neighbours of the GEMM: ``act_fn(gate_proj(x)) * up_proj(x)`` of a Llama-style MLP in ONE
 launch with the SiLU-mul in the epilogue (module order in the reference's model definitions:
-/root/reference/gptqmodel/models/definitions/llama.py:17-27 — gate_proj and up_proj are separate QuantLinear modules whose
+gptqmodel/models/definitions/llama.py:17-27 — gate_proj and up_proj are separate QuantLinear modules whose
 outputs a Python expression combines: two matmul launches, one activation launch, one multiply launch).
 
 The kernel is the two-weight-set mode of the small-batch tier (b2q_midm.cu MODE 1, the same launch the grouped MoE path uses
-with one "expert"): both weight sets run through the pipeline back to back into two TMEM accumulators, the epilogue rounds
+with one "expert"): both weight sets run through the pipeline back to back into two register accumulators, the epilogue rounds
 at the module boundaries exactly like the separate modules would (g = T(x W_gate), a = T(silu(g)), u = T(x W_up),
 h = T(a * u)) and stores h only — the two [M, intermediate] intermediates never reach HBM.  Serves 1 <= tokens <= 128 per
 call (larger batches: `forward` falls back to the two modules' own tiers + torch ops).

@@ -1,8 +1,8 @@
-"""Mixture-of-experts block over QuantLinear experts (BASELINE configs[4]: Mixtral-8x7B int4 g64 asym; SURVEY.md §8e).
+"""Mixture-of-experts block over QuantLinear experts (BASELINE configs[4]: Mixtral-8x7B int4 g64 asym).
 
 In the reference every expert's ``w1 / w3 / w2`` is an independent QuantLinear module
-(/root/reference/gptqmodel/models/definitions/mixtral.py:30-34) that the model's own Python loop calls per expert; the
-fused MoE kernel it ships (``swordfish_moe.cu``) is exported but never called (SURVEY.md §2b).  This module is that
+(gptqmodel/models/definitions/mixtral.py:30-34) that the model's own Python loop calls per expert; the
+fused MoE kernel it ships (``swordfish_moe.cu``) is exported but never called.  This module is that
 per-expert loop, arranged for the B200 kernels and for tensor parallelism:
 
   * ONE TOKEN (batch-1 decode) through grouped-eligible experts: three launches on the decode tier — the 2 * top_k gate / up
@@ -53,9 +53,9 @@ class MoEExperts(torch.nn.Module):
         self.group = group
         self.reduce = reduce  # optional tp.P2PAllReduce for decode-sized outputs
         self.decode_path = True  # one token: the decode-tier launches (False: always the grouped small-batch kernels; A/B)
-        # SiLU-mul folded into the down launch's activation staging (two launches instead of three).  OFF: measured slower on
-        # the Mixtral TP-4 shard stack (723 vs 758 tok/s, profiles/r02_moe_decode_notes.md) — every CTA of a rank recomputes the
-        # row's exp() on the critical path between the PDL wait and its first mma, while the separate 2 us kernel overlaps
+        # SiLU-mul folded into the down launch's activation staging (two launches instead of three).  OFF by default: every
+        # CTA of a rank recomputes the row's exp() on the critical path between the PDL wait and its first mma, while the
+        # separate small kernel overlaps
         self.fuse_act = False
         self._stack = None
         if grouped is None or grouped:

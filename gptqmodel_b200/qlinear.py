@@ -1,6 +1,6 @@
-"""B200QuantLinear — drop-in GPTQ QuantLinear whose forward() runs hand-written sm_100a CUDA.
+"""B200QuantLinear — drop-in GPTQ QuantLinear whose forward() runs hand-written sm_90a (H100) CUDA.
 
-Mirrors the class contract of the reference's kernels (SURVEY.md §8b):
+Mirrors the class contract of the reference's kernels:
   constructor / buffers : gptqmodel/nn_modules/qlinear/__init__.py:664-692, 827-865 (qweight, qzeros, scales, g_idx,
                           bias in CHECKPOINT layout so a loader can fill them), qlinear/swordfish.py:66-148
   capability attributes : qlinear/swordfish.py:40-62 / qlinear/marlin.py:59-75 (`SUPPORTS_*`, REQUIRES_FORMAT_V2)
@@ -41,8 +41,7 @@ class SiblingGroup:
     The first member called with a new `x` launches for all members and parks the siblings'
     outputs; each sibling's `forward(x)` then just picks its result up.  Every module keeps the reference's
     per-module `forward(x) -> y` contract (same arithmetic; bit-identical to separate calls whenever the fused launch
-    splits K like the single launches would, see `b2q_debug_decode_plan`); only the launch count changes.  This is
-    SURVEY.md §8 row f1 ("fused neighbours of the GEMM").
+    splits K like the single launches would, see `b2q_debug_decode_plan`); only the launch count changes.
 
     Contract: parked outputs are keyed on (data_ptr, version, M, dtype) of the activations, are handed out once, and
     are dropped as soon as any member is called with different activations.  The group keeps a strong reference to the
@@ -531,8 +530,8 @@ class B200QuantLinear(B200KernelMixin, nn.Module):
         if not torch.cuda.is_available():
             return False, NotImplementedError("B200QuantLinear needs a CUDA device")
         major, minor = torch.cuda.get_device_capability()
-        if major != 10:
-            return False, NotImplementedError(f"B200QuantLinear is built for sm_100a only, found sm_{major}{minor}")
+        if (major, minor) != (9, 0):
+            return False, NotImplementedError(f"B200QuantLinear is built for sm_90a only, found sm_{major}{minor}")
         return True, None
 
     @classmethod

@@ -17,8 +17,8 @@ in their own `__dict__` (gptqmodel/utils/importer.py:110-127), ranks them by the
   * `post_init()` / `forward()` / `dequantize_weight()` / `list_buffers()` come from the mixin; `post_init()` ends in the
     base's `post_init()` (adapter initialisation, qlinear/__init__.py:224-234).
 The file a maintainer adds is shown in INTEGRATION.md §2; tests/test_reference_shim.py builds the class against a
-stand-in hierarchy with the reference's exact constructor signatures and, when /root/reference is present, against the
-unmodified reference classes themselves.
+stand-in hierarchy with the reference's exact constructor signatures and against what the shim did on the unmodified
+reference classes (tests/golden/shim_reference.json, written by tests/golden/check_shim.py --write).
 """
 from __future__ import annotations
 
@@ -74,8 +74,8 @@ def make_reference_kernel(base_cls, *, backend, methods, formats, adapters, devi
             if not torch.cuda.is_available():
                 return False, NotImplementedError(f"{cls.__name__} needs a CUDA device")
             major, minor = torch.cuda.get_device_capability()
-            if major != 10:
-                return False, NotImplementedError(f"{cls.__name__} is built for sm_100a only, found sm_{major}{minor}")
+            if (major, minor) != (9, 0):
+                return False, NotImplementedError(f"{cls.__name__} is built for sm_90a only, found sm_{major}{minor}")
             return True, None
 
     _B200Linear.__name__ = _B200Linear.__qualname__ = class_name

@@ -1,6 +1,6 @@
 """Tensor-parallel sharding of GPTQ QuantLinear checkpoint tensors + the row-parallel all-reduce.
 
-The reference has no tensor-parallel code (SURVEY.md §2c); the rules below are the ones it documents for the
+The reference has no tensor-parallel code; the rules below are the ones it documents for the
 engines it delegates to: scales of a row-parallel act-order layer must be replicated on all ranks
 (`marlin_repeat_scales_on_all_ranks`, gptqmodel/utils/marlin.py:300-305), K shards must be whole groups
 (`marlin_is_k_full` :296-297, TensorParallelPadderConfig quantization/config.py:1184-1188).
@@ -103,7 +103,7 @@ def shard_rows(layer: Layer, rank: int, world: int) -> Layer:
 
 
 def shard_moe_expert(w1: Layer, w3: Layer, w2: Layer, rank: int, world: int):
-    """One expert of a Mixtral-style MoE block under tensor parallelism (SURVEY.md §8e, BASELINE configs[4]):
+    """One expert of a Mixtral-style MoE block under tensor parallelism (BASELINE configs[4]):
     w1 / w3 (gate / up) column-parallel, w2 (down) row-parallel — every rank keeps a slice of EVERY expert, so the block
     needs one all-reduce of the combined output, exactly like a dense MLP."""
     return shard_columns(w1, rank, world), shard_columns(w3, rank, world), shard_rows(w2, rank, world)
@@ -253,9 +253,8 @@ class RowParallelLinear(torch.nn.Module):
         """Prefill-sized inputs: the token rows are cut into `overlap_chunks` blocks (multiples of the 256-row GEMM tile);
         the NCCL all-reduce of block c runs on a side stream while the shard's GEMM of block c + 1 runs on the caller's
         stream, so only the last block's collective is exposed.  Fork / join with events: CUDA-graph capturable.  OPT-IN
-        (`overlap_chunks` > 1): measured at TP-4 it is SLOWER than one GEMM + one all-reduce (17.5 vs 12.3 ms per 2048-token
-        pass: the quarter-size GEMMs fill the 74 CTA pairs worse, NCCL competes for SMs with the GEMM it overlaps, and the
-        blocks are concatenated afterwards) — profiles/r02_tp_notes.md."""
+        (`overlap_chunks` > 1): the smaller GEMMs fill the SMs worse, NCCL competes for SMs with the GEMM it overlaps, and the
+        blocks are concatenated afterwards, so it can be slower than one GEMM + one all-reduce."""
         M = x2.shape[0]
         cs = -(-M // self.overlap_chunks)
         cs = max(256, (cs + 255) // 256 * 256)

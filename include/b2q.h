@@ -1,4 +1,4 @@
-/* b2q.h — C ABI of libb2q.so: the B200-native (sm_100a) GPTQ W4A16/W8A16 QuantLinear hot path.
+/* b2q.h — C ABI of libb2q.so: the H100-native (sm_90a) GPTQ W4A16/W8A16 QuantLinear hot path.
  *
  * This is the boundary a host framework binds (ctypes / cffi / a torch.library shim); no torch or C++ types cross
  * it.  All pointers are DEVICE pointers unless noted, all calls are asynchronous on `stream` (a cudaStream_t passed
@@ -57,8 +57,8 @@ int b2q_prepack(const int32_t* qweight, const int32_t* perm, void* packed, int K
 /* out[M, N] = x[M, K] @ dequant(W) (+ bias).  Dispatches on M inside the library so a CUDA graph sees the true M:
  *   M <= 8 (4-bit, group 64|128|K)  : decode tier (mma.sync, cluster split-K)           b2q_decode.cu
  *   M == 1 (8-bit)                  : CUDA-core GEMV                                     b2q_gemv.cu
- *   M <= 128 otherwise              : small-batch tier (swapped tcgen05 operands, cluster split-K)  b2q_midm.cu
- *   M  > 128                        : CTA-pair tcgen05 prefill tier (4-bit) / single-CTA tier (8-bit)
+ *   M <= 128 otherwise              : small-batch tier (swapped wgmma operands, cluster split-K)  b2q_midm.cu
+ *   M  > 128                        : wgmma prefill tier                                         b2q_gemm.cu
  * The call runs on the device that owns `packed`, whatever the caller's current device is.
  *   x, scales, bias, out : fp16 (dtype 0) or bf16 (dtype 1), all the same type; x and out contiguous row-major
  *   qzeros               : NULL for symmetric layers (zero-point 2^(bits-1)), else int32 [G, N*bits/32]
@@ -73,7 +73,7 @@ int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t*
  *   b2q_decode : 4-bit, 1 <= M <= 8, K % 128 == 0, group_size 64|128|K: fragment-major weights -> mma.sync, per-group
  *                fix-up, cluster split-K reduced through distributed shared memory (the bs=1 decode path)
  *   b2q_gemv   : M == 1 (routes 4-bit to b2q_decode, 8-bit to the CUDA-core fma.rn.f32.f16 GEMV)
- *   b2q_gemm   : any M, the tcgen05 + TMA tensor-core tier */
+ *   b2q_gemm   : any M, the wgmma + TMA tensor-core tiers */
 int b2q_decode(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
                const void* bias, void* out, int M, int K, int N, int bits, int group_size, int dtype, int ks,
                int warps, void* stream);
@@ -147,7 +147,7 @@ int b2q_moe_decode_down(const void* h, const void* packed2, const void* scales2,
                         int group_size, int dtype, int fused_act, void* y, void* stream);
 
 /* In-place all-reduce(sum) of a small 16-bit vector (n % 8 == 0, n <= max_elems) across `world` <= 8 GPUs of one
- * NVLink domain: the single collective of a row-parallel QuantLinear at decode time (SURVEY.md §8e; the reference has
+ * NVLink domain: the single collective of a row-parallel QuantLinear at decode time (the reference has
  * none).  peer_bufs is a HOST array of `world` device pointers to every rank's symmetric buffer (this rank's included),
  * each laid out as data[2][world][max_elems] (16-bit) followed at byte `flag_offset` by flags[2][world] (u32),
  * zero-initialised once; `seq` is a device u32[2] owned by this rank, zero-initialised once: {call counter, status}.  Every
@@ -157,7 +157,7 @@ int b2q_allreduce(void* inout, int n, int dtype, int rank, int world, const void
                   int max_elems, void* seq, void* stream);
 
 /* Row-parallel QuantLinear shard AND its all-reduce(sum) in ONE launch (decode tier: bits = 4, 1 <= M <= 8, no
- * act-order; SURVEY.md §8e — the reference has no collective).  Every rank calls it with its K-shard (x [M, K/world],
+ * act-order — the reference has no collective).  Every rank calls it with its K-shard (x [M, K/world],
  * weights of those rows) and the same M, N; the kernel pushes its fp32 partial sums into every rank's symmetric buffer
  * over NVLink peer memory, exchanges per-CTA flags, sums the `world` partials in rank order and stores
  * out[M, N] = round(sum_r x_r @ dequant(W_r) (+ bias)) on every rank.  Pass the bias on ONE rank only
@@ -167,7 +167,7 @@ int b2q_allreduce(void* inout, int n, int dtype, int rank, int world, const void
  *                 >= 2*world*max_elems*4) u32 flags of b2q_decode_allreduce_flag_bytes() bytes; zero-initialised once
  *   ctl         : this rank's device u32[4] {sequence, arrivals, status (1 + rank of a peer that timed out), -}, zeroed once
  * Every rank must issue the same sequence of calls with the same shapes.  CUDA-graph safe (nothing is reset).
- * EXPERIMENTAL in round 1: compiled, not yet validated on GPUs (DESIGN.md §6b). */
+ * EXPERIMENTAL: validated only by tools/tp_fused_smoke.py on several GPUs, not by the single-GPU suite. */
 int b2q_decode_allreduce(const void* x, const void* packed, const void* scales, const int32_t* qzeros,
                          const void* bias, void* out, int M, int K, int N, int bits, int group_size, int dtype,
                          int rank, int world, const void* const* peer_bufs, size_t flag_offset, int max_elems,
@@ -178,7 +178,7 @@ size_t b2q_decode_allreduce_flag_bytes(void);
  * call path). */
 void b2q_debug_reload_env(void);
 
-/* Debug: device buffer (>= 148*16 uint64) receiving %globaltimer phase stamps of the decode kernel; NULL = off. */
+/* Debug: device buffer (>= 160*16 uint64) receiving %globaltimer phase stamps of the decode kernel; NULL = off. */
 void b2q_debug_set_trace(void* device_buffer);
 
 /* Debug / tests (host only, no GPU needed): the launch plan the decode tier would use for out[M, N] with N the total

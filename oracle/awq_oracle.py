@@ -2,7 +2,7 @@
 
 Restates (no code copied) what the reference computes for an AWQ GEMM-format layer:
   * layout: ``qweight int32 [K, N*bits/32]`` packed along the OUTPUT dimension, ``qzeros int32 [G, N*bits/32]`` packed the
-    same way, ``scales fp16 [G, N]`` (/root/reference/gptqmodel/nn_modules/qlinear/__init__.py:1634-1668);
+    same way, ``scales fp16 [G, N]`` (gptqmodel/nn_modules/qlinear/__init__.py:1634-1668);
   * inside every 32-bit word the 8 nibbles are interleaved: nibble i (bits 4i..4i+3) holds logical column
     8c + AWQ_ORDER[i], AWQ_ORDER = [0, 2, 4, 6, 1, 3, 5, 7]; reading logical column j means nibble
     AWQ_REVERSE_ORDER[j] = [0, 4, 1, 5, 2, 6, 3, 7][j] (quantization/awq/utils/packing_utils.py:9-10, 43-58);

@@ -14,7 +14,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: pytest -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
 
 
 def pytest_sessionfinish(session, exitstatus):
-    """On a GPU box: dump the worst err/tol ratio every parity test observed (profiles/r02_parity.json is a copy)."""
+    """On a GPU box: dump the worst err/tol ratio every parity test observed (to $B2Q_PARITY_JSON)."""
     if not torch.cuda.is_available():
         return
     try:

@@ -1,8 +1,11 @@
 #!/usr/bin/env python
-"""Authoring-container check (needs /root/reference): build gptqmodel_b200.reference_shim's class on the UNMODIFIED
-reference base `GPTQQuantLinear`, construct it the way `create_quant_module` does (gptqmodel/utils/model.py:630-647), and
-run the reference's own discovery walk over it.  Prints one JSON line; tests/test_reference_shim.py runs it in a
-subprocess so the stubbed third-party modules never leak into the test process.
+"""Check against a GPTQModel checkout (see make_golden.py for how it is located): build gptqmodel_b200.reference_shim's
+class on the UNMODIFIED reference base `GPTQQuantLinear`, construct it the way `create_quant_module` does
+(gptqmodel/utils/model.py:630-647), and run the reference's own discovery walk over it.  Prints one JSON line;
+
+    python tests/golden/check_shim.py --write
+
+also writes it to tests/golden/shim_reference.json, the fixture tests/test_reference_shim.py compares against.
 """
 import json
 import os
@@ -92,3 +95,7 @@ m5 = B200Linear(bits=5, group_size=64, desc_act=False, sym=False, in_features=25
 out["bits3"] = dict(qweight=list(m3.qweight.shape), qzeros=list(m3.qzeros.shape), kbits=m3.kbits, planar=bool(m3.planar))
 out["bits5"] = dict(qweight=list(m5.qweight.shape), qzeros=list(m5.qzeros.shape), kbits=m5.kbits, planar=bool(m5.planar))
 print("SHIM_JSON " + json.dumps(out))
+if "--write" in sys.argv:
+    rec = {"source": "tests/golden/check_shim.py: gptqmodel_b200.reference_shim on the unmodified GPTQModel classes", **out}
+    with open(os.path.join(HERE, "shim_reference.json"), "w") as f:
+        json.dump(rec, f, indent=1, sort_keys=True)

@@ -35,7 +35,7 @@ import transformers.modeling_utils  # noqa: E402,F401
 
 from unittest.mock import MagicMock  # noqa: E402
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("GPTQMODEL_SRC") or "/root/reference"
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

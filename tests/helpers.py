@@ -7,7 +7,7 @@ import oracle
 def make_layer(K, N, bits=4, group_size=128, sym=True, desc_act=False, bias=False, seed=42, dtype=torch.float16):
     """Returns dict of CPU checkpoint-layout tensors (v2 qzeros) quantised from randn weights.
 
-    Recipe follows SURVEY.md §8(d): W = randn(N, K, seed) * 0.5, sym grid of tests/kernels/test_swordfish.py:31-56
+    Recipe: W = randn(N, K, seed) * 0.5, sym grid of tests/kernels/test_swordfish.py:31-56
     or min/max asym, act-order g_idx = (arange // g)[randperm].
     """
     gen = torch.Generator().manual_seed(seed)

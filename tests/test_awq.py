@@ -1,4 +1,4 @@
-"""AWQ (FORMAT.GEMM) front-end (SURVEY.md §8 row f3): oracle pinned to the reference, exact layout conversion, GPU parity.
+"""AWQ (FORMAT.GEMM) front-end: oracle pinned to the reference, exact layout conversion, GPU parity.
 
 Fixtures: tests/golden/awq_cases.npz, produced by running the UNMODIFIED reference's `dequantize_gemm` and
 `AwqTorchLinear.forward` (tests/golden/make_golden_awq.py).
@@ -49,7 +49,7 @@ def test_scale_once_arithmetic_vs_per_weight_rounding(awq_cases):
     kernel that applies the scale once per group to an exact integer dot product is the same sum without those K
     roundings.  On the reference's own fixture `awq_gK` (K = 128, one group, M = 2) even float64-exact arithmetic lands
     1.18x outside `1e-3*|ref| + 1e-3*rms(ref)` of the rounded-W oracle on one of the 256 outputs — the very element and
-    ratio the round-1 GPU run reported for the decode tier (GPUTEST_r01.json) — so that miss was the reference's
+    ratio an earlier GPU run reported for the decode tier — so that miss was the reference's
     weight-rounding noise, not kernel arithmetic; with the 4-sigma noise term every case is inside."""
     from helpers import PARITY_LOG, ref_rounding_slack  # noqa: F401
     worst = {}

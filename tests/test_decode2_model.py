@@ -60,7 +60,7 @@ def simulate(M, K, N, p):
         prev_end = b
     assert off["xbar"][1] <= p["smem"] <= 200 * 1024, (off, p)
     assert off["sx"][0] % 16 == 0 and off["bars"][0] % 8 == 0 and off["wpart"][0] % 4 == 0
-    assert C_cta * ks <= 148
+    assert C_cta * ks <= 132
 
     units = {}    # (tile, quad) -> count
     emitted = {}  # (m, n) -> count

@@ -210,7 +210,7 @@ SMALL_BATCH_CASES = [
 
 @pytest.mark.parametrize("K,N,bits,gs,sym,desc,bias", SMALL_BATCH_CASES)
 def test_small_batch_tier_matches_oracle(K, N, bits, gs, sym, desc, bias):
-    """b2q_midm.cu (swapped tcgen05 operands + cluster split-K): every token-box width (16/32/64/128), partial boxes,
+    """b2q_midm.cu (swapped wgmma operands + cluster split-K): every token-box width (16/32/64/128), partial boxes,
     every split-K cluster size, through the module and the raw ABI."""
     import gptqmodel_b200 as g
     import os
@@ -401,7 +401,7 @@ def test_sibling_fusion_with_shared_act_order():
     (8192, 3584, "gate/up column shard"), (3584, 8192, "down_proj row shard"),
 ])
 def test_llama3_70b_tp8_shard_shapes(K, N, kind):
-    """BASELINE configs[3]: the per-rank QuantLinear shapes of Llama-3-70B under TP-8 (SURVEY.md §8d), decode + prefill."""
+    """BASELINE configs[3]: the per-rank QuantLinear shapes of Llama-3-70B under TP-8, decode + prefill."""
     L = random_layer(K, N, bits=4, group_size=128, sym=True, seed=K * 7 + N)
     mod = _module(L)
     W = oracle.dequantize_weight(L["qweight"].to(DEV), L["qzeros"].to(DEV), L["scales"].to(DEV),

@@ -1,4 +1,4 @@
-"""GPU parity of the format front-ends (SURVEY.md §8 rows f3 / f2): AWQ GEMM-format modules against outputs produced
+"""GPU parity of the format front-ends: AWQ GEMM-format modules against outputs produced
 by the reference's own AwqTorchLinear, full-size AWQ layers against the oracle, and a checkpoint loaded from safetensors.
 
 Lives in its own file so that it is collected AFTER tests/test_gpu_parity.py (the hot path proper).
@@ -136,7 +136,7 @@ def test_moe_block_on_gpu(T):
 @pytest.mark.gpu
 @pytest.mark.parametrize("sym,gs", [(True, 128), (False, 64)])
 def test_fused_gate_up_silu_epilogue_on_gpu(sym, gs):
-    # SURVEY §8 row f1: act_fn(gate_proj(x)) * up_proj(x) in one launch, SiLU-mul in the epilogue, rounding at the module
+    # act_fn(gate_proj(x)) * up_proj(x) in one launch, SiLU-mul in the epilogue, rounding at the module
     # boundaries of the reference's separate modules
     import torch.nn.functional as F
     from gptqmodel_b200 import B200QuantLinear

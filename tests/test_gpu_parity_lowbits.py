@@ -1,5 +1,5 @@
 """GPU parity of the widened layouts (2 / 3-bit, planar 3 / 5 / 6 / 7-bit), arbitrary g_idx and act-order row shards
-(SURVEY.md §8 row f4, VERDICT r01 items 9 / 10).  Outputs are compared with (a) what the UNMODIFIED reference produced for
+(VERDICT r01 items 9 / 10).  Outputs are compared with (a) what the UNMODIFIED reference produced for
 the same checkpoint tensors (tests/golden/lowbit_cases.npz) and (b) the oracle on larger layers at every kernel tier."""
 import json
 import os
@@ -65,7 +65,7 @@ def test_lowbit_layers_at_every_tier(bits, planar, gs, sym, desc_act):
                                                   desc_act=desc_act, sym=sym, format="gptq_p" if planar else "gptq_v2")
     W = oracle.dequantize_weight_any(L["qweight"], L["qzeros"], L["scales"], L["g_idx"], bits, planar)
     gen = torch.Generator().manual_seed(bits)
-    for M in (1, 5, 16, 100, 300):  # decode / GEMV, small-batch tcgen05, prefill tiers
+    for M in (1, 5, 16, 100, 300):  # decode / GEMV, small-batch wgmma, prefill tiers
         x = (torch.randn(M, K, generator=gen) * 0.5).to(torch.float16)
         ref = oracle.forward_any(x, L["qweight"], L["qzeros"], L["scales"], L["g_idx"], bits, planar)
         assert_close_rel(mod(x.cuda()), ref, 1e-3, f"{bits}-bit planar={planar} g{gs} M={M}",

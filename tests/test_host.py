@@ -85,7 +85,7 @@ def test_checkpoint_buffer_shapes_match_reference_layout():
     m8 = B200QuantLinear(bits=8, group_size=-1, desc_act=False, sym=True, in_features=256, out_features=64)
     assert m8.qweight.shape == (64, 64) and m8.qzeros.shape == (1, 16) and m8.group_size == 256
     sd = m.state_dict()
-    assert set(sd) == {"qweight", "qzeros", "scales", "g_idx", "bias"}  # the wire format (SURVEY §5)
+    assert set(sd) == {"qweight", "qzeros", "scales", "g_idx", "bias"}  # the wire format
 
 
 def test_no_cpu_fallback():
@@ -120,7 +120,7 @@ def test_decode_launch_plan_invariants(version):
                     continue
                 C, pks, pw, gw, qpc, max_tiles, stages, smem = list(out)
                 quads, tiles = K // 128, N // 32
-                assert 1 <= C and C * pks <= 148 and pks in (1, 2, 4, 8) and pw in (4, 8, 16), list(out)
+                assert 1 <= C and C * pks <= 132 and pks in (1, 2, 4, 8) and pw in (4, 8, 16), list(out)
                 assert pw % gw == 0 and stages in (2, 4) and smem <= 200 * 1024, list(out)
                 assert qpc * pks >= quads and (pks - 1) * qpc < quads, list(out)  # every rank owns >= 1 quad
                 ngroups = pw // gw

@@ -1,7 +1,7 @@
 """2 / 3-bit continuous and planar 3 / 5 / 6 / 7-bit checkpoint layouts, exact widening, arbitrary g_idx (CPU).
 
 Pinned against tensors packed, dequantised and multiplied by the UNMODIFIED reference (tests/golden/lowbit_cases.npz,
-generator tests/golden/make_golden_lowbits.py): /root/reference/gptqmodel/nn_modules/qlinear/__init__.py:946-1003,
+generator tests/golden/make_golden_lowbits.py): gptqmodel/nn_modules/qlinear/__init__.py:946-1003,
 utils/planar_packing.py.  The oracle (numpy bit matrices) and the product (torch field tables) are independent
 restatements; both must reproduce the reference bit for bit.
 """

@@ -1,4 +1,4 @@
-"""Checkpoint loader (SURVEY.md §8 row f2): config spellings, dynamic overrides, v1 -> v2 zero-points, sharded files.
+"""Checkpoint loader: config spellings, dynamic overrides, v1 -> v2 zero-points, sharded files.
 
 Host-side only: tiny synthetic checkpoints are written with safetensors and loaded onto the CPU without post_init();
 the tensors the modules end up holding are compared with the oracle (dequantised weights must survive the trip).

@@ -13,7 +13,7 @@ META = json.loads(bytes(np.load(os.path.join(GOLDEN, "ref_cases.npz"))["__meta__
 
 
 def test_q4_reference_golden_vector(q4_golden):
-    # recipe: /root/reference/tests/test_q4_exllama_v2.py:32-87, vector: tests/q4_reference.py
+    # recipe: GPTQModel tests/test_q4_exllama_v2.py:32-87, vector: tests/q4_reference.py
     torch.manual_seed(42)
     qweight = torch.randint(-100, 100, size=(128, 1024), dtype=torch.int32)
     scales = torch.zeros(8, 1024, dtype=torch.float16) + 0.002

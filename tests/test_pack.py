@@ -1,4 +1,4 @@
-"""Device-side packer (SURVEY.md §8 row f4) against the reference's own packers.
+"""Device-side packer against the reference's own packers.
 
 tests/golden/ref_cases.npz holds, for every case, the float weights, the [N, G] scale / zero grids and the tensors the
 reference's `pack_block` AND `pack_original` produced (asserted identical when the fixture was generated,

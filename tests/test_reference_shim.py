@@ -5,13 +5,12 @@ class called a cooperative `super().__init__()` with no arguments.  Two checks:
   1. against a STAND-IN hierarchy that restates the reference's constructor signatures (qlinear/__init__.py:102-194,
      664-692, 727-760), its `validate()` plumbing (:257-332) and the discovery walk + priority ranking of
      utils/importer.py:110-127,182-233 — runs everywhere;
-  2. against the UNMODIFIED reference classes (tests/golden/check_shim.py in a subprocess) — only where /root/reference
-     exists (the authoring container).
+  2. against what the shim did on the UNMODIFIED reference classes: tests/golden/check_shim.py ran it there once and
+     its answers are stored in tests/golden/shim_reference.json; the stand-in-based shim must give the same answers.
 """
 import copy
 import json
 import os
-import subprocess
 import sys
 from typing import Optional
 
@@ -207,14 +206,10 @@ def test_standalone_class_still_has_the_whole_contract():
     assert m.qzero_format() == 2 and m.qzeros.shape == (2, 8)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/gptqmodel"), reason="the reference tree is only mounted in the "
-                    "authoring container")
 def test_shim_against_the_unmodified_reference_classes():
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "golden", "check_shim.py")], capture_output=True,
-                       text=True, timeout=600)
-    line = [ln for ln in r.stdout.splitlines() if ln.startswith("SHIM_JSON ")]
-    assert line, r.stdout[-2000:] + r.stderr[-4000:]
-    out = json.loads(line[-1][len("SHIM_JSON "):])
+    with open(os.path.join(ROOT, "tests", "golden", "shim_reference.json")) as f:
+        out = json.load(f)
+    # what the reference classes answered (recorded)
     assert out["mro"][:3] == ["B200Linear", "B200KernelMixin", "GPTQQuantLinear"]
     assert out["verify_supports_params"] and out["discovered"] and out["constructed"] and out["isinstance_base"]
     assert out["top_for_gptq"] == "B200Linear"
@@ -224,3 +219,25 @@ def test_shim_against_the_unmodified_reference_classes():
     assert out["bits3"] == dict(qweight=[24, 128], qzeros=[2, 12], kbits=4, planar=False)
     assert out["bits5"] == dict(qweight=[40, 128], qzeros=[4, 20], kbits=8, planar=True)
     assert out["state_dict_keys"] == ["bias", "g_idx", "qweight", "qzeros", "scales"]
+    # the same construction on the stand-in hierarchy gives the same answers
+    cls = _make()
+    assert [c.__name__ for c in cls.__mro__[:2]] == out["mro"][:2]
+    cls.validate_once = classmethod(lambda c: (True, None))
+    m = cls(bits=4, group_size=128, desc_act=False, sym=True, in_features=256, out_features=128,
+            pack_dtype=torch.int32, bias=True, dtype=torch.float16, name=out["name"], lm_head_name="lm_head",
+            backend="gptq_b200", register_buffers=True, adapter=None)
+    assert {k: list(getattr(m, k).shape) for k in out["shapes"]} == out["shapes"]
+    assert m.qzero_format() == out["qzeros_format_initial"]
+    assert sorted(m.state_dict()) == out["state_dict_keys"] and len(m.list_buffers()) == out["n_list_buffers"]
+    with pytest.raises(NotImplementedError):
+        cls(bits=16, group_size=128, desc_act=False, sym=True, in_features=256, out_features=128,
+            pack_dtype=torch.int32, bias=False, backend="gptq_b200", adapter=None)
+    m3 = cls(bits=3, group_size=128, desc_act=False, sym=True, in_features=256, out_features=128,
+             pack_dtype=torch.int32, bias=False, backend="gptq_b200", adapter=None, register_buffers=True)
+    assert dict(qweight=list(m3.qweight.shape), qzeros=list(m3.qzeros.shape), kbits=m3.kbits,
+                planar=bool(m3.planar)) == out["bits3"]
+    m5 = cls(bits=5, group_size=64, desc_act=False, sym=False, in_features=256, out_features=128,
+             pack_dtype=torch.int32, bias=False, backend="gptq_b200", adapter=None, register_buffers=True,
+             format="gptq_p")
+    assert dict(qweight=list(m5.qweight.shape), qzeros=list(m5.qzeros.shape), kbits=m5.kbits,
+                planar=bool(m5.planar)) == out["bits5"]

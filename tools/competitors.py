@@ -1,10 +1,10 @@
-"""Competitor kernels on the SAME box, SAME packed checkpoint tensors (VERDICT r01 row g, SURVEY §8d baselines 2-3).
+"""Competitor kernels on the SAME box, SAME packed checkpoint tensors (VERDICT r01 row g).
 
   python tools/competitors.py [--json gpurun_out/competitors.json] [--quick]
 
 Arms (each reported as available / unavailable with the reason):
-  * "marlin_ref"  — the reference's own Marlin (gptqmodel_ext/marlin) compiled by baseline/build_marlin.py from the sources
-                    under /root/reference into baseline/_ref/ (git-ignored, travels with gpurun); call sequence restates
+  * "marlin_ref"  — the reference's own Marlin (gptqmodel_ext/marlin) compiled by oracle/build_marlin.py from a GPTQModel
+                    checkout into oracle/_ref/ (git-ignored); call sequence restates
                     MarlinLinear.post_init / forward (qlinear/marlin.py:246-337, utils/marlin.py:471-608).
   * "marlin_vllm" — vLLM 0.22's build of the same kernel family (torch.ops._C.marlin_gemm): library code in the image.
   * "cublas_fp16" — dense fp16 torch.matmul on the dequantised weights (context only: 4x the bytes at M=1).
@@ -64,7 +64,7 @@ class MarlinVllm:
         from vllm.model_executor.layers.quantization.utils import marlin_utils as mu
         from vllm.scalar_type import scalar_types
         self.ops, self.mu, self.st = ops, mu, scalar_types
-        self.ws = torch.zeros(148 * 4, dtype=torch.int32, device="cuda")
+        self.ws = torch.zeros(132 * 4, dtype=torch.int32, device="cuda")
         self.empty = torch.empty(0, dtype=torch.int32, device="cuda")
         self.info = f"vllm {__import__('vllm').__version__} torch.ops._C.marlin_gemm (import {time.time() - t0:.0f}s)"
 
@@ -81,20 +81,20 @@ class MarlinVllm:
 
 
 class MarlinRef:
-    """The reference's Marlin, built by baseline/build_marlin.py (op schema: marlin_torch_fp16.cpp)."""
+    """The reference's Marlin, built by oracle/build_marlin.py (op schema: marlin_torch_fp16.cpp)."""
     name = "marlin_ref"
 
     def __init__(self):
-        so = os.path.join(ROOT, "baseline", "_ref", "gptqmodel_marlin_fp16.so")
+        so = os.path.join(ROOT, "oracle", "_ref", "gptqmodel_marlin_fp16.so")
         if not os.path.exists(so):
-            raise RuntimeError(f"{so} not built (python baseline/build_marlin.py in the authoring container)")
+            raise RuntimeError(f"{so} not built (GPTQMODEL_SRC=<GPTQModel checkout> python oracle/build_marlin.py)")
         torch.ops.load_library(so)
         self.ns = torch.ops.gptqmodel_marlin_fp16
         # workspace: int32[max(SMs, 128)] zeros (utils/marlin.py:308-319)
         self.ws = torch.zeros(max(torch.cuda.get_device_properties(0).multi_processor_count, 128) * 4,
                               dtype=torch.int32, device="cuda")
         self.empty = torch.empty(0, dtype=torch.int32, device="cuda")
-        self.info = "reference gptqmodel_ext/marlin compiled for sm_100a (baseline/build_marlin.py)"
+        self.info = "reference gptqmodel_ext/marlin compiled for sm_90a (oracle/build_marlin.py)"
 
     @staticmethod
     def _permute_scales(s, K, N, gs):

@@ -2,7 +2,7 @@
 
   python tools/microbench.py gemv     sweep split-K cluster size / warps per Llama-3-8B shape (M=1)
   python tools/microbench.py gemv2    same sweep for the experimental decode kernel v2 (+ warps per tile group), vs v1
-  python tools/microbench.py gemm     time the tcgen05 GEMM at M=2048 per shape
+  python tools/microbench.py gemm     time the wgmma GEMM at M=2048 per shape
 """
 import json
 import os
@@ -58,7 +58,7 @@ def gemv(MB=1):
     p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
     for K, N in SHAPES:
         nbytes = K * N // 2
-        copies = max(2, int(300e6 // nbytes) + 1)  # rotate > L2 (126 MB) of distinct weights
+        copies = max(2, int(300e6 // nbytes) + 1)  # rotate > L2 (50 MB) of distinct weights
         if os.environ.get("MB_L2") == "1":
             copies = 1  # weights stay L2-resident: measures latency chain + L2 streaming
         mods = build(K, N, copies)

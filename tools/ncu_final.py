@@ -38,7 +38,7 @@ torch.cuda.synchronize()
 torch.cuda.profiler.start()
 for name, mods in cases:
     mods[-1](xs[mods[-1].in_features])   # the layer not touched during warm-up: HBM-cold weights
-cases[2][1][-1](xp)                      # act-order prefill: permute_rows_kernel + gemm2p_kernel
+cases[2][1][-1](xp)                      # act-order prefill: permute_rows_kernel + gemm_kernel
 torch.cuda.synchronize()
 torch.cuda.profiler.stop()
 print("captured", [c[0] for c in cases], "+ act-order prefill")

@@ -32,5 +32,5 @@ for r in rows[2:]:
     out.append("tensor pipes: " + "; ".join(tensor[:6]))
 text = "\n".join(out)
 if len(sys.argv) > 2:
-    open(sys.argv[2], "w").write(f"# {rep} (ncu --set full --clock-control none; B200)\n" + text + "\n")
+    open(sys.argv[2], "w").write(f"# {rep} (ncu --set full --clock-control none)\n" + text + "\n")
 print(text[:3000])

@@ -12,7 +12,7 @@ for c in range(12):
     L = random_layer(K, N, seed=c, device="cuda")
     mods.append(B200QuantLinear.from_checkpoint_tensors(L["qweight"], L["qzeros"], L["scales"], L["g_idx"], 4, 128, device="cuda"))
 x = (torch.randn(1, K, device="cuda") * 0.5).to(torch.float16)
-traces = [torch.zeros(148 * 16, dtype=torch.int64, device="cuda") for _ in mods]
+traces = [torch.zeros(160 * 16, dtype=torch.int64, device="cuda") for _ in mods]
 def fn():
     for m, tr in zip(mods, traces):
         g.lib.b2q_debug_set_trace(tr.data_ptr())
@@ -25,7 +25,7 @@ gr = torch.cuda.CUDAGraph()
 with torch.cuda.graph(gr): fn()
 for _ in range(3): gr.replay()
 torch.cuda.synchronize()
-T = torch.stack(traces).cpu().reshape(len(mods), 148, 16).double()
+T = torch.stack(traces).cpu().reshape(len(mods), 160, 16).double()
 base = T[6][:, 0].min()
 for li in (6, 7):
     t = T[li] - base
