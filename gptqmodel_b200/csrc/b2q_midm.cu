@@ -40,7 +40,7 @@ constexpr int MM_RED_WARPS = 8;             // warps 0..7 reduce the split-K par
 // latency: with 4 stages (the first version of this kernel) only 16 KB of weights per SM were in flight and every k-block
 // cost one HBM round trip / 4; Little's law asks for tens of KB in flight per SM.  The DEQUANTISED ring (WST stages of 16 KB) only
 // decouples the dequant warps from the tensor core.
-// MODE 0: one QuantLinear.  MODE 1 / 2: GROUPED over the experts of a MoE block (b2q_moe.cu): blockIdx.z = (expert, token
+// MODE 0: one QuantLinear.  MODE 1 / 2: GROUPED over the experts of a MoE block (b2q_moe.cu): z0 + blockIdx.z = (expert, token
 // block); the rows of an expert are contiguous in the expert-sorted activation matrix; CTAs beyond an expert's row count
 // exit at once.  MODE 1 runs TWO weight sets (w1 = gate, w3 = up) through the pipeline back to back into two register
 // accumulators and stores silu(gate) * up; MODE 2 (w2 = down) scales each row by its routing weight and scatters it to the
@@ -54,7 +54,9 @@ struct MoeArgs {
   const void* scales3;
   const uint32_t* qzeros3;
   float* ypair;                 // [rows, N] fp32, row = pair index                                   (MODE 2)
-  int tblocks;                  // token blocks (of NTOK rows) per expert in gridDim.z
+  int tblocks;                  // token blocks (of NTOK rows) per expert
+  int z0;                       // (expert, token block) index of blockIdx.z == 0: launch_midm_grouped splits a grid
+                                // of more than 65535 such blocks into several launches
 };
 
 template <int BITS, int NTOK, int PST, int WST, int MODE = 0>
@@ -94,7 +96,8 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
   if (MODE != 0) {
     // the routing tables are written by the preceding kernel of the stream: nothing may be read before it has finished
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int e = (int)blockIdx.z / G.tblocks, tb = (int)blockIdx.z - e * G.tblocks;
+    const int z = G.z0 + (int)blockIdx.z;
+    const int e = z / G.tblocks, tb = z - e * G.tblocks;
     const int cnt = G.counts[e];
     if (tb * NTOK >= cnt) return;  // same decision in every CTA of the cluster (they differ in blockIdx.y only)
     row0 = G.offsets[e] + tb * NTOK;
@@ -583,7 +586,7 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   // (mode 1 holds two accumulator sets in the registers of the MMA warpgroup: blocks of at most 64 tokens)
   const int ntok = g.rows <= 16 ? 16 : g.rows <= 32 ? 32 : (g.rows <= 64 || mode == 1) ? 64 : 128;
   G.tblocks = (g.rows + ntok - 1) / ntok;
-  const int grid_z = g.E * G.tblocks;
+  const long long total_z = (long long)g.E * G.tblocks;
   int ks = env().midm_ks > 0 ? env().midm_ks : midm_grouped_ranks(a.K, a.N, g.active > 0 ? g.active : 1);
   if (ks > 8) ks = 8;
   const int nkb = a.K / MM_BK;
@@ -597,7 +600,20 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
 #define B2Q_MG_CASE(T)                                                                       \
   (mode == 1 ? (asym ? B2Q_MG_NTOK(T, true, 1) : B2Q_MG_NTOK(T, false, 1))                   \
              : (asym ? B2Q_MG_NTOK(T, true, 2) : B2Q_MG_NTOK(T, false, 2)))
-  return a.dtype == 0 ? B2Q_MG_CASE(__half) : B2Q_MG_CASE(__nv_bfloat16);
+  // gridDim.z is at most 65535 on every CUDA device: a prefill chunk of a many-expert block (E = 128, top_k = 8: 8T/64
+  // token blocks per expert in MODE 1, i.e. from T = 4089 on) needs more (expert, token block) pairs than that, so the grid
+  // is issued as consecutive launches over ranges of z; a grid that fits is one launch with z0 = 0, as before.  Chained
+  // launches stay ordered under programmatic dependent launch: every CTA of MODE 1 / 2 executes griddepcontrol.wait (the
+  // previous grid has completed and its writes are visible) before it can exit, so a launch completes only after all the
+  // launches before it, and the next kernel's wait on the last launch covers them all.
+  constexpr int MAX_Z = 65535;
+  for (long long z0 = 0; z0 < total_z; z0 += MAX_Z) {
+    G.z0 = (int)z0;
+    const int grid_z = (int)(total_z - z0 < MAX_Z ? total_z - z0 : MAX_Z);
+    const int e = a.dtype == 0 ? B2Q_MG_CASE(__half) : B2Q_MG_CASE(__nv_bfloat16);
+    if (e != 0) return e;
+  }
+  return 0;
 #undef B2Q_MG_CASE
 #undef B2Q_MG_NTOK
 }

@@ -72,20 +72,22 @@ __global__ void __launch_bounds__(128)
 
 template <typename T>
 __global__ void __launch_bounds__(256)
-    moe_combine_kernel(const float* __restrict__ ypair, T* __restrict__ y, int top_k, int N) {
+    moe_combine_kernel(const float* __restrict__ ypair, T* __restrict__ y, int ntokens, int top_k, int N) {
   using E = ET<T>;
-  const int t = blockIdx.y;
   const int n = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (n >= N) return;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int j = 0; j < top_k; ++j) {
-    const float4 v = *reinterpret_cast<const float4*>(ypair + ((size_t)t * top_k + j) * N + n);
-    acc.x += v.x;
-    acc.y += v.y;
-    acc.z += v.z;
-    acc.w += v.w;
+  // tokens stride by gridDim.y (at most 65535): one pass for every T the grid covers, more for longer inputs
+  for (int t = blockIdx.y; t < ntokens; t += gridDim.y) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = 0; j < top_k; ++j) {
+      const float4 v = *reinterpret_cast<const float4*>(ypair + ((size_t)t * top_k + j) * N + n);
+      acc.x += v.x;
+      acc.y += v.y;
+      acc.z += v.z;
+      acc.w += v.w;
+    }
+    *reinterpret_cast<uint2*>(y + (size_t)t * N + n) = make_uint2(E::pack2(acc.x, acc.y), E::pack2(acc.z, acc.w));
   }
-  *reinterpret_cast<uint2*>(y + (size_t)t * N + n) = make_uint2(E::pack2(acc.x, acc.y), E::pack2(acc.z, acc.w));
 }
 
 int launch_moe_align(const int32_t* topk_ids, int T, int top_k, int E, int32_t* counts, int32_t* offsets,
@@ -105,9 +107,9 @@ int launch_moe_gather(const void* x, const int32_t* sorted_pairs, void* xs, int 
 }
 
 int launch_moe_combine(const float* ypair, void* y, int T, int top_k, int N, int dtype, cudaStream_t stream) {
-  dim3 grid((N / 4 + 255) / 256, T, 1);
-  if (dtype == 0) moe_combine_kernel<__half><<<grid, 256, 0, stream>>>(ypair, (__half*)y, top_k, N);
-  else moe_combine_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(ypair, (__nv_bfloat16*)y, top_k, N);
+  dim3 grid((N / 4 + 255) / 256, T < 65535 ? T : 65535, 1);
+  if (dtype == 0) moe_combine_kernel<__half><<<grid, 256, 0, stream>>>(ypair, (__half*)y, T, top_k, N);
+  else moe_combine_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(ypair, (__nv_bfloat16*)y, T, top_k, N);
   return (int)cudaGetLastError();
 }
 
