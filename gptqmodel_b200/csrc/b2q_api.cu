@@ -433,10 +433,24 @@ int b2q_moe_gather(const void* x, const int32_t* sorted_pairs, void* xs, int row
   return check_cuda(launch_moe_gather(x, sorted_pairs, xs, rows, top_k, K, (cudaStream_t)stream), "b2q_moe_gather");
 }
 
+int b2q_moe_gather_perm(const void* src, const int32_t* sorted_pairs, const int32_t* perms, const int32_t* offsets, int E,
+                        void* dst, int rows, int top_k, int K, void* stream) {
+  if (src == nullptr || perms == nullptr || offsets == nullptr || dst == nullptr || E < 1 || rows < 1 || top_k < 1 ||
+      K < 8 || K % 8 != 0 || (reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 15) ||
+      (reinterpret_cast<uintptr_t>(perms) & 15)) {
+    set_error("b2q_moe_gather_perm: bad argument (E=%d rows=%d top_k=%d K=%d; K %% 8 == 0, 16-byte aligned)", E, rows,
+              top_k, K);
+    return -2;
+  }
+  DeviceGuard dg(dst);
+  return check_cuda(launch_moe_gather_perm(src, sorted_pairs, perms, offsets, E, dst, rows, top_k, K, (cudaStream_t)stream),
+                    "b2q_moe_gather_perm");
+}
+
 static int moe_check(const char* fn, const void* x, const void* packed, const void* scales, const int32_t* counts,
                      const int32_t* offsets, int E, int rows, int K, int N, int bits, int group_size, int dtype) {
-  if (counts == nullptr || offsets == nullptr || E < 1 || rows < 1 || bits != 4) {
-    set_error("%s: bad argument (E=%d rows=%d bits=%d; the grouped path serves 4-bit experts)", fn, E, rows, bits);
+  if (counts == nullptr || offsets == nullptr || E < 1 || rows < 1 || (bits != 4 && bits != 8)) {
+    set_error("%s: bad argument (E=%d rows=%d bits=%d; the grouped path serves 4- and 8-bit experts)", fn, E, rows, bits);
     return -2;
   }
   return validate(fn, x, packed, scales, x, rows, K, N, bits, group_size, dtype);

@@ -71,6 +71,8 @@ int launch_moe_align(const int32_t* topk_ids, int T, int top_k, int E, int32_t* 
                      int32_t* sorted_pairs, cudaStream_t stream);
 int launch_moe_gather(const void* x, const int32_t* sorted_pairs, void* xs, int rows, int top_k, int K,
                       cudaStream_t stream);
+int launch_moe_gather_perm(const void* src, const int32_t* sorted_pairs, const int32_t* perms, const int32_t* offsets,
+                           int E, void* dst, int rows, int top_k, int K, cudaStream_t stream);
 int launch_moe_combine(const float* ypair, void* y, int T, int top_k, int N, int dtype, cudaStream_t stream);
 int launch_moe_decode_gate_up(const MmArgs& a, const void* packed1, const void* scales1, const int32_t* qzeros1,
                               const void* packed3, const void* scales3, const int32_t* qzeros3, const int32_t* ids,

@@ -74,7 +74,6 @@ struct MidCfg {
   static constexpr int ACC = NTOK / 2;                   // fp32 accumulator registers per thread, per set and m64 block
   static_assert(NSETS * NTOK <= 128, "accumulators of the MMA warpgroup: at most 128 registers per thread");
   static constexpr int PART_BYTES = NSETS * NTOK * MM_BF * 4;  // fp32 partial tile(s) [set][token][feature]
-  static_assert(MODE == 0 || BITS == 4, "the grouped (MoE) modes are built for 4-bit experts");
   static_assert(X_BYTES % 1024 == 0, "x tiles must stay 1024-byte aligned (SWIZZLE_128B atoms)");
   static_assert(PART_BYTES <= RING_BYTES, "the fp32 partial tile reuses the idle stage buffers");
   static_assert((PST + 2 * XST + 2 * WST) * 8 <= BAR_BYTES, "mbarrier area");
@@ -103,14 +102,16 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
     row0 = G.offsets[e] + tb * NTOK;
     M = min(NTOK, cnt - tb * NTOK);
     const size_t groups = (size_t)(K >> 5) >> gshc;  // quantisation groups along K (gshc = log2(32-k chunks per group))
-    const size_t wstride = (size_t)K * N / 32, sstride = (gshc >= 31 ? 1 : groups) * (size_t)N;
+    // one expert: K*N*BITS/8 bytes of codes (uint4 units), G*N scales, G*N/(32/BITS) zero words
+    const size_t wstride = (size_t)K * N / (128 / BITS), sstride = (gshc >= 31 ? 1 : groups) * (size_t)N;
+    const size_t zstride = sstride / (32 / BITS);
     packed += (size_t)e * wstride;
     scales += (size_t)e * sstride;
-    if (ASYM) qzeros += (size_t)e * (sstride >> 3);
+    if (ASYM) qzeros += (size_t)e * zstride;
     if (MODE == 1) {
       packed_b = G.packed3 + (size_t)e * wstride;
       scales_b = reinterpret_cast<const T*>(G.scales3) + (size_t)e * sstride;
-      if (ASYM) qzeros_b = G.qzeros3 + (size_t)e * (sstride >> 3);
+      if (ASYM) qzeros_b = G.qzeros3 + (size_t)e * zstride;
     }
   }
   extern __shared__ uint8_t smem_raw[];
@@ -346,13 +347,16 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
       // two uint4 (16 k each) per (row, half)
       constexpr int R = (128 / TG) > 0 ? 128 / TG : 1;  // (TG = 256 only exists for the 4-bit debug variant)
       for (int i = gq; i < NI; i += DQG) {
-        const int kb = kb0 + i, s = i % PST, ws = i % WST;
+        const bool second = NSETS > 1 && i >= nkb;  // MODE 1: iterations nkb.. stream the second weight set
+        const int kb = kb0 + (second ? i - nkb : i), s = i % PST, ws = i % WST;
+        const T* sc = second ? scales_b : scales;
+        const uint32_t* zq = second ? qzeros_b : qzeros;
         SZRaw sz[R][2];
 #pragma unroll
         for (int r = 0; r < R; ++r) {
           const int n = n0 + tl + TG * r;
 #pragma unroll
-          for (int j = 0; j < 2; ++j) sz[r][j] = load_sz<T, BITS, ASYM>(scales, qzeros, (2 * kb + j) >> gshc, n < N ? n : 0, N);
+          for (int j = 0; j < 2; ++j) sz[r][j] = load_sz<T, BITS, ASYM>(sc, zq, (2 * kb + j) >> gshc, n < N ? n : 0, N);
         }
         mbar_wait(bar_pfull + 8 * s, (i / PST) & 1);
         uint4 pvs[R][2][2];
@@ -567,9 +571,10 @@ int midm_grouped_ranks(int K, int N, int active) {
 }
 
 int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
-  if (a.bits != 4 || a.K % MM_BK != 0 || a.N % 32 != 0 || (mode != 1 && mode != 2) || g.E < 1 || g.rows < 1) {
-    set_error("b2q_moe: grouped launch needs bits=4, K %% 64 == 0, N %% 32 == 0 (bits=%d K=%d N=%d E=%d rows=%d)", a.bits,
-              a.K, a.N, g.E, g.rows);
+  if ((a.bits != 4 && a.bits != 8) || a.K % MM_BK != 0 || a.N % 32 != 0 || (mode != 1 && mode != 2) || g.E < 1 ||
+      g.rows < 1) {
+    set_error("b2q_moe: grouped launch needs bits 4 or 8, K %% 64 == 0, N %% 32 == 0 (bits=%d K=%d N=%d E=%d rows=%d)",
+              a.bits, a.K, a.N, g.E, g.rows);
     return -1;
   }
   MoeArgs G = {};
@@ -592,11 +597,18 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   const int nkb = a.K / MM_BK;
   while (ks > 1 && (ks - 1) * ((nkb + ks - 1) / ks) >= nkb) ks >>= 1;
   const bool asym = a.qzeros != nullptr;
-#define B2Q_MG_NTOK(T, AS, MODE)                                                             \
+  // packed-ring depths per token block: those of B2Q_MM_NTOK (launch_midm) for the same bit width
+#define B2Q_MG_NTOK4(T, AS, MODE)                                                            \
   (ntok == 16   ? launch_midm_t<T, 4, AS, 16, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
    : ntok == 32 ? launch_midm_t<T, 4, AS, 32, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
    : ntok == 64 ? launch_midm_t<T, 4, AS, 64, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
                 : launch_midm_t<T, 4, AS, (MODE == 1 ? 64 : 128), (MODE == 1 ? 8 : 4), 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
+#define B2Q_MG_NTOK8(T, AS, MODE)                                                            \
+  (ntok == 16   ? launch_midm_t<T, 8, AS, 16, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
+   : ntok == 32 ? launch_midm_t<T, 8, AS, 32, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
+   : ntok == 64 ? launch_midm_t<T, 8, AS, 64, 4, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
+                : launch_midm_t<T, 8, AS, (MODE == 1 ? 64 : 128), 4, 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
+#define B2Q_MG_NTOK(T, AS, MODE) (a.bits == 4 ? B2Q_MG_NTOK4(T, AS, MODE) : B2Q_MG_NTOK8(T, AS, MODE))
 #define B2Q_MG_CASE(T)                                                                       \
   (mode == 1 ? (asym ? B2Q_MG_NTOK(T, true, 1) : B2Q_MG_NTOK(T, false, 1))                   \
              : (asym ? B2Q_MG_NTOK(T, true, 2) : B2Q_MG_NTOK(T, false, 2)))
@@ -616,6 +628,8 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   return 0;
 #undef B2Q_MG_CASE
 #undef B2Q_MG_NTOK
+#undef B2Q_MG_NTOK8
+#undef B2Q_MG_NTOK4
 }
 
 }  // namespace b2q

@@ -10,7 +10,10 @@
 //                         h[i, :] = silu(xs[i] W1_e) * (xs[i] W3_e)      both weight sets in ONE launch, SiLU-mul epilogue
 //   4. midm_kernel<MODE 2>: ypair[pair(i), :] = w[pair(i)] * (h[i] W2_e)  routing weight + scatter to the pair's slot
 //   5. moe_combine_kernel y[t, :] = sum_j ypair[t*k + j, :]               fp32 sum, ONE rounding, deterministic
-// Expert weights are the prepacked B2Q tensors of the per-expert QuantLinears, stacked (expert stride = one tensor).
+// Expert weights are the prepacked B2Q tensors of the per-expert QuantLinears, stacked (expert stride = one tensor), 4- or
+// 8-bit.  Act-order experts were prepacked with their rows in group order, so each expert reads its activations in its
+// own column order: moe_gather_perm_kernel replaces step 2 (xs[i, k'] = x[sorted_pairs[i] / k, P13_e[k']]) and, when w2
+// has act-order, permutes h between steps 3 and 4 (h2[i, k'] = h[i, P2_e[k']]).
 #include "b2q_common.cuh"
 #include "b2q_internal.h"
 
@@ -70,6 +73,38 @@ __global__ void __launch_bounds__(128)
   for (int j = threadIdx.x; j < k16; j += blockDim.x) dst[j] = src[j];
 }
 
+// act-order experts: one CTA per sorted row i, dst[i, k'] = src[r(i), perms[e(i) * K + k']] with r(i) = sorted_pairs[i] /
+// top_k (or i when sorted_pairs is NULL) and e(i) the expert whose sorted rows hold i.  16-bit elements gathered from the
+// source row (it stays in L1 / L2), stored as 16-byte vectors.
+__global__ void __launch_bounds__(128)
+    moe_gather_perm_kernel(const uint16_t* __restrict__ src, const int32_t* __restrict__ sorted_pairs,
+                           const int32_t* __restrict__ perms, const int32_t* __restrict__ offsets, int E,
+                           uint4* __restrict__ dst, int top_k, int K) {
+  const int i = blockIdx.x;
+  // upper bound of i over offsets, minus one: the last expert whose first row is <= i (an expert without rows has the
+  // offset of the next one, so the search passes over it)
+  int lo = 0, hi = E;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (offsets[mid] <= i) lo = mid + 1;
+    else hi = mid;
+  }
+  const int e = lo > 0 ? lo - 1 : 0;
+  const int r = sorted_pairs != nullptr ? sorted_pairs[i] / top_k : i;
+  const uint16_t* s = src + (size_t)r * K;
+  const int4* p = reinterpret_cast<const int4*>(perms + (size_t)e * K);
+  uint4* d = dst + (size_t)i * (K / 8);
+  for (int j = threadIdx.x; j < K / 8; j += blockDim.x) {
+    const int4 a = p[2 * j], b = p[2 * j + 1];
+    uint4 o;
+    o.x = (uint32_t)__ldg(s + a.x) | ((uint32_t)__ldg(s + a.y) << 16);
+    o.y = (uint32_t)__ldg(s + a.z) | ((uint32_t)__ldg(s + a.w) << 16);
+    o.z = (uint32_t)__ldg(s + b.x) | ((uint32_t)__ldg(s + b.y) << 16);
+    o.w = (uint32_t)__ldg(s + b.z) | ((uint32_t)__ldg(s + b.w) << 16);
+    d[j] = o;
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
     moe_combine_kernel(const float* __restrict__ ypair, T* __restrict__ y, int ntokens, int top_k, int N) {
@@ -103,6 +138,17 @@ int launch_moe_align(const int32_t* topk_ids, int T, int top_k, int E, int32_t* 
 int launch_moe_gather(const void* x, const int32_t* sorted_pairs, void* xs, int rows, int top_k, int K,
                       cudaStream_t stream) {
   moe_gather_kernel<<<rows, 128, 0, stream>>>((const uint4*)x, sorted_pairs, (uint4*)xs, top_k, K / 8);
+  return (int)cudaGetLastError();
+}
+
+int launch_moe_gather_perm(const void* src, const int32_t* sorted_pairs, const int32_t* perms, const int32_t* offsets,
+                           int E, void* dst, int rows, int top_k, int K, cudaStream_t stream) {
+  if (E > MOE_MAX_EXPERTS) {
+    set_error("b2q_moe_gather_perm: at most %d experts (got %d)", MOE_MAX_EXPERTS, E);
+    return -1;
+  }
+  moe_gather_perm_kernel<<<rows, 128, 0, stream>>>((const uint16_t*)src, sorted_pairs, perms, offsets, E, (uint4*)dst,
+                                                   top_k, K);
   return (int)cudaGetLastError();
 }
 

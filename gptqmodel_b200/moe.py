@@ -5,16 +5,22 @@ In the reference every expert's ``w1 / w3 / w2`` is an independent QuantLinear m
 fused MoE kernel it ships (``swordfish_moe.cu``) is exported but never called.  This module is that
 per-expert loop, arranged for the B200 kernels and for tensor parallelism:
 
-  * ONE TOKEN (batch-1 decode) through grouped-eligible experts: three launches on the decode tier — the 2 * top_k gate / up
-    matrices as sibling sets of one decode launch (experts read from `topk_ids` on the device), SiLU-mul, and a cluster of
-    top_k CTAs per tile column for w2 whose DSMEM reduction applies the routing weights (`b2q_moe_decode_*`);
-  * GROUPED path (default whenever every expert is a 4-bit B200 QuantLinear of one shape): the (token, k) pairs are sorted
-    by expert ON THE DEVICE (`b2q_moe_align`), and the whole block is five launches with no host synchronisation —
-    align, gather, ONE grouped launch for w1 and w3 with the SiLU-mul epilogue, ONE grouped launch for w2 with the routing
-    weight + scatter epilogue, combine (gptqmodel_b200/csrc/b2q_moe.cu, grouped modes of b2q_midm.cu) — CUDA-graph
-    capturable; the experts' prepacked tensors are stacked once (the per-expert modules keep views into the stack);
-  * LOOP path (fallback: dense stand-ins in CPU tests, mixed experts): tokens are sorted by expert once, every expert sees one
-    contiguous block of its routed tokens; one host sync per block for the per-expert counts, like the reference's loop;
+  * ONE TOKEN (batch-1 decode) through grouped-eligible 4-bit experts without act-order: three launches on the decode tier —
+    the 2 * top_k gate / up matrices as sibling sets of one decode launch (experts read from `topk_ids` on the device),
+    SiLU-mul, and a cluster of top_k CTAs per tile column for w2 whose DSMEM reduction applies the routing weights
+    (`b2q_moe_decode_*`); other grouped-eligible stacks take the grouped path at one token as well;
+  * GROUPED path (default whenever every expert is a B200 QuantLinear of one shape, see `_build_stack`): the (token, k)
+    pairs are sorted by expert ON THE DEVICE (`b2q_moe_align`), and the whole block is five launches with no host
+    synchronisation — align, gather, ONE grouped launch for w1 and w3 with the SiLU-mul epilogue, ONE grouped launch for w2
+    with the routing weight + scatter epilogue, combine (gptqmodel_b200/csrc/b2q_moe.cu, grouped modes of b2q_midm.cu) —
+    CUDA-graph capturable; the experts' prepacked tensors are stacked once (the per-expert modules keep views into the
+    stack).  Experts are 4- or 8-bit in the kernels (2 / 3 / 5 / 6 / 7-bit checkpoints are widened exactly by post_init), one
+    width for w1 / w3 and one for w2.  Act-order experts were prepacked with their rows in group order: the gather reads
+    each expert's activations in that expert's column order (`b2q_moe_gather_perm`), and a w2 with act-order gets h
+    permuted the same way before the down launch (six launches);
+  * LOOP path (fallback: dense stand-ins in CPU tests, mixed experts, regrouped act-order shards): tokens are sorted by
+    expert once, every expert sees one contiguous block of its routed tokens; one host sync per block for the per-expert
+    counts, like the reference's loop;
   * tensor parallel: ``w1 / w3`` column-sharded, ``w2`` row-sharded (`tp.shard_moe_expert`), so every rank holds a slice
     of EVERY expert and the block ends in exactly one all-reduce of the combined output, as for a dense MLP.
 
@@ -61,8 +67,10 @@ class MoEExperts(torch.nn.Module):
         if grouped is None or grouped:
             self._stack = self._build_stack()
             if grouped and self._stack is None:
-                raise ValueError("MoEExperts(grouped=True): experts must be post_init'ed 4-bit B200 QuantLinears of one "
-                                 "shape / group size without act-order, bias or adapters")
+                raise ValueError("MoEExperts(grouped=True): experts must be post_init'ed B200 QuantLinears of one shape / "
+                                 "group size, with one kernel bit width (4 or 8) for w1 / w3 and one for w2, the same "
+                                 "act-order permutation in w1 and w3 of every expert, and no regrouped g_idx, bias or "
+                                 "adapters")
         if fuse and self._stack is None:
             from .qlinear import B200KernelMixin, fuse_siblings
 
@@ -78,36 +86,59 @@ class MoEExperts(torch.nn.Module):
         for mods in (self.w1, self.w3, self.w2):
             m0 = mods[0]
             for m in mods:
-                if not isinstance(m, B200KernelMixin) or not m._prepacked or m.bits != 4 or m.perm is not None or m._gather is not None \
+                # kbits: the 4- or 8-bit container the kernels stream (post_init widens other widths exactly); a
+                # regrouped g_idx (unequal groups) gathers and pads x per layer, which the stacked launches cannot do
+                if not isinstance(m, B200KernelMixin) or not m._prepacked or m.kbits not in (4, 8) or m._gather is not None \
                         or m.bias is not None or m.adapter:
                     return None
-                if (m.in_features, m.out_features, m.group_size, m.packed.device, m.scales.dtype) != (
-                        m0.in_features, m0.out_features, m0.group_size, m0.packed.device, m0.scales.dtype):
+                if (m.in_features, m.out_features, m.group_size, m.kbits, m.packed.device, m.scales.dtype) != (
+                        m0.in_features, m0.out_features, m0.group_size, m0.kbits, m0.packed.device, m0.scales.dtype):
                     return None
             sets.append(list(mods))
         w1, w3, w2 = sets
-        if (w1[0].in_features, w1[0].out_features, w1[0].group_size) != (w3[0].in_features, w3[0].out_features,
-                                                                         w3[0].group_size):
+        if (w1[0].in_features, w1[0].out_features, w1[0].group_size, w1[0].kbits) != (
+                w3[0].in_features, w3[0].out_features, w3[0].group_size, w3[0].kbits):
             return None
         if w2[0].in_features != w1[0].out_features:
             return None
+        # w1 and w3 of an expert read the same gathered activations: they must share the act-order permutation (true of
+        # real checkpoints, where both are quantised against the same inputs)
+        for a, b in zip(w1, w3):
+            if (a.perm is None) != (b.perm is None) or (a.perm is not None and not torch.equal(a.perm, b.perm)):
+                return None
         out = {}
         for name, mods in (("w1", w1), ("w3", w3), ("w2", w2)):
             asym = any(not m._is_sym for m in mods) if name == "w2" else any(not m._is_sym for m in w1 + w3)
             packed = torch.stack([m.packed for m in mods]).contiguous()
             scales = torch.stack([m.scales.data for m in mods]).contiguous()
-            zeros = torch.stack([m.qzeros.data for m in mods]).contiguous() if asym else None
+            zeros = torch.stack([self._kernel_zeros(m) for m in mods]).contiguous() if asym else None
             for e, m in enumerate(mods):  # the modules keep working on their own; no second copy of the weights
                 m.packed = packed[e]
                 m.scales.data = scales[e]
                 m._scales_cache.clear()
                 if zeros is not None:
-                    m.qzeros.data = zeros[e]
+                    if m.kbits == m.bits:  # a widened module's qzeros keeps the checkpoint's narrower fields
+                        m.qzeros.data = zeros[e]
                     if m._zeros_dev is not None:
                         m._zeros_dev = zeros[e]
+            perm = None  # [E, K]: the order half of every expert's permutation, the identity where there is none
+            if any(m.perm is not None for m in mods):
+                K = mods[0].in_features
+                ident = torch.arange(K, dtype=torch.int32, device=packed.device)
+                perm = torch.stack([ident if m.perm is None else m.perm[:K] for m in mods]).contiguous()
             out[name] = dict(packed=packed, scales={scales.dtype: scales}, zeros=zeros, K=mods[0].in_features,
-                             N=mods[0].out_features, group=mods[0].group_size)
+                             N=mods[0].out_features, group=mods[0].group_size, bits=mods[0].kbits, perm=perm)
         return out
+
+    @staticmethod
+    def _kernel_zeros(m):
+        """The zero points of one expert in the layout the kernels read (int32 [G, N * kbits / 32]): the widened tensor of
+        an asymmetric module, the kbits symmetric word for a symmetric one."""
+        if m._zeros_dev is not None:
+            return m._zeros_dev
+        zsym = {4: 0x88888888 - (1 << 32), 8: 0x80808080 - (1 << 32)}[m.kbits]
+        return torch.full((m.scales.shape[0], m.out_features * m.kbits // 32), zsym, dtype=torch.int32,
+                          device=m.packed.device)
 
     def _scales(self, name, dtype):
         d = self._stack[name]["scales"]
@@ -155,22 +186,32 @@ class MoEExperts(torch.nn.Module):
         y = torch.empty((T, Kout), dtype=dt, device=dev)
         active = min(E, rows)
         check(lib.b2q_moe_align(p(ids), T, top_k, E, p(counts), p(offsets), p(sorted_pairs), st), "b2q_moe_align")
-        check(lib.b2q_moe_gather(p(x2), p(sorted_pairs), p(xs), rows, top_k, K, st), "b2q_moe_gather")
+        if s1["perm"] is None:
+            check(lib.b2q_moe_gather(p(x2), p(sorted_pairs), p(xs), rows, top_k, K, st), "b2q_moe_gather")
+        else:  # act-order w1 / w3: every expert's rows gathered in its own column order
+            check(lib.b2q_moe_gather_perm(p(x2), p(sorted_pairs), p(s1["perm"]), p(offsets), E, p(xs), rows, top_k, K, st),
+                  "b2q_moe_gather_perm")
         check(lib.b2q_moe_gate_up(p(xs), p(s1["packed"]), p(self._scales("w1", dt)), p(s1["zeros"]), p(s3["packed"]),
                                   p(self._scales("w3", dt)), p(s3["zeros"]), p(h), p(counts), p(offsets), E, rows, active,
-                                  K, inter, 4, s1["group"], code, st), "b2q_moe_gate_up")
+                                  K, inter, s1["bits"], s1["group"], code, st), "b2q_moe_gate_up")
+        if s2["perm"] is not None:  # act-order w2: h permuted per expert (its rows are already in expert order)
+            h2 = torch.empty_like(h)
+            check(lib.b2q_moe_gather_perm(p(h), None, p(s2["perm"]), p(offsets), E, p(h2), rows, top_k, inter, st),
+                  "b2q_moe_gather_perm")
+            h = h2
         check(lib.b2q_moe_down(p(h), p(s2["packed"]), p(self._scales("w2", dt)), p(s2["zeros"]), p(counts), p(offsets),
-                               p(sorted_pairs), p(wts), p(ypair), E, rows, active, inter, Kout, 4, s2["group"], code, st),
-              "b2q_moe_down")
+                               p(sorted_pairs), p(wts), p(ypair), E, rows, active, inter, Kout, s2["bits"], s2["group"],
+                               code, st), "b2q_moe_down")
         check(lib.b2q_moe_combine(p(ypair), p(y), T, top_k, Kout, code, st), "b2q_moe_combine")
         return y
 
     def _decode_ok(self, top_k: int) -> bool:
-        """The decode tier's envelope for the one-token path: K % 128 == 0 on both matmuls, group_size 64 / 128 / K,
-        top_k in {2, 4, 8} (cluster size of the down launch)."""
+        """The decode tier's envelope for the one-token path: 4-bit experts without act-order, K % 128 == 0 on both
+        matmuls, group_size 64 / 128 / K, top_k in {2, 4, 8} (cluster size of the down launch)."""
         s1, s2 = self._stack["w1"], self._stack["w2"]
         ok_g = lambda s: s["group"] in (64, 128, s["K"])  # noqa: E731
-        return (top_k in (2, 4, 8) and s1["K"] % 128 == 0 and s2["K"] % 128 == 0 and s1["N"] % 32 == 0
+        return (top_k in (2, 4, 8) and s1["bits"] == 4 and s2["bits"] == 4 and s1["perm"] is None
+                and s2["perm"] is None and s1["K"] % 128 == 0 and s2["K"] % 128 == 0 and s1["N"] % 32 == 0
                 and s2["N"] % 32 == 0 and ok_g(s1) and ok_g(s2))
 
     @property

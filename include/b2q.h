@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 3
+#define B2Q_ABI_VERSION 4
 #define B2Q_DTYPE_F16 0
 #define B2Q_DTYPE_BF16 1
 
@@ -106,10 +106,18 @@ int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const vo
 /* ---- Grouped MoE expert path (BASELINE configs[4]; the reference's unused analogue: swordfish_moe.cu:9-17,38-48) --------
  * y[t] = sum_j w[t, j] * W2_e( silu(W1_e x[t]) * W3_e x[t] ),  e = topk_ids[t, j], in FIVE launches without any host
  * synchronisation (CUDA-graph capturable).  Expert weights are the b2q_prepack'ed tensors of the per-expert QuantLinears
- * STACKED along a leading expert dimension (packed [E][K*N/2 bytes], scales [E][G][N], qzeros [E][G][N/8] or NULL when every
- * expert is symmetric); 4-bit, any supported group size, no act-order.  rows = T * top_k (token, j) pairs; pair p = t*top_k+j.
+ * STACKED along a leading expert dimension (packed [E][K*N*bits/8 bytes], scales [E][G][N], qzeros [E][G][N*bits/32] or NULL
+ * when every expert is symmetric); bits 4 or 8 (one width per stack, gate_up and down may differ), any supported group
+ * size.  rows = T * top_k (token, j) pairs; pair p = t*top_k+j.
  *   b2q_moe_align   : topk_ids int32 [T, top_k] -> counts [E], offsets [E], sorted_pairs [rows] (stable by expert)
  *   b2q_moe_gather  : xs [rows, K]  <- x[sorted_pairs[i] / top_k]
+ *   b2q_moe_gather_perm : act-order experts (prepacked with their rows in group order) read their activations in their own
+ *                     column order; this replaces b2q_moe_gather (perms = P13 [E, K], the order half of each expert's w1
+ *                     permutation, w3 sharing it; the identity for an expert without act-order) and, when w2 has act-order,
+ *                     permutes h before b2q_moe_down (sorted_pairs = NULL, perms = P2 [E, N of gate_up]):
+ *                       dst[i, k'] = src[r(i), perms[e(i) * K + k']],  r(i) = sorted_pairs[i] / top_k (or i when
+ *                       sorted_pairs == NULL),  e(i) = the last expert e with offsets[e] <= i (the expert whose sorted rows
+ *                       hold i).  16-bit elements, E <= 256, K % 8 == 0; src, dst and perms 16-byte aligned, dst != src.
  *   b2q_moe_gate_up : h [rows, N]   <- silu(xs W1_e) * (xs W3_e), both weight sets in one launch (rounded to the 16-bit
  *                     dtype at every module boundary of the reference's per-expert loop); `active` = experts expected to
  *                     receive rows (grid sizing only, e.g. min(E, rows))
@@ -118,6 +126,8 @@ int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const vo
 int b2q_moe_align(const int32_t* topk_ids, int T, int top_k, int E, int32_t* counts, int32_t* offsets,
                   int32_t* sorted_pairs, void* stream);
 int b2q_moe_gather(const void* x, const int32_t* sorted_pairs, void* xs, int rows, int top_k, int K, void* stream);
+int b2q_moe_gather_perm(const void* src, const int32_t* sorted_pairs, const int32_t* perms, const int32_t* offsets,
+                        int E, void* dst, int rows, int top_k, int K, void* stream);
 int b2q_moe_gate_up(const void* xs, const void* packed1, const void* scales1, const int32_t* qzeros1,
                     const void* packed3, const void* scales3, const int32_t* qzeros3, void* h, const int32_t* counts,
                     const int32_t* offsets, int E, int rows, int active, int K, int N, int bits, int group_size, int dtype,
