@@ -25,15 +25,10 @@ static EnvCfg read_env() {
   EnvCfg c;
   c.disable_pdl = env_int("B2Q_DISABLE_PDL", 0);
   c.midm = env_int("B2Q_MIDM", 1);
-  c.decode_blocks_m = env_int("B2Q_DECODE_BLOCKS_M", 0);
-  c.decode_groups2 = env_int("B2Q_DECODE_GROUPS", 1) == 2;
   c.decode_v2 = env_int("B2Q_DECODE_V2", -1);
   c.decode2_gw = env_int("B2Q_DECODE2_GW", 0);
-  c.decode2_ks = env_int("B2Q_DECODE2_KS", 0);
   c.decode2_xtma = env_int("B2Q_DECODE2_XTMA", 0);
-  c.decode2_fastsync = env_int("B2Q_DECODE2_FASTSYNC", 0);
   c.midm_ks = env_int("B2Q_MIDM_KS", 0);
-  c.midm_dqg1 = env_int("B2Q_MIDM_DQG1", 0);
   return c;
 }
 
@@ -144,8 +139,6 @@ using namespace b2q;
 extern "C" {
 
 int b2q_version(void) { return B2Q_ABI_VERSION; }
-
-void b2q_debug_set_trace(void* device_buffer) { g_trace_ptr = device_buffer; }
 
 int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, int* out8) {
   if (out8 == nullptr || (version != 1 && version != 2) || M < 1 || M > 8 || K < 128 || K % 128 != 0 || N < 32 ||
@@ -389,23 +382,6 @@ int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t*
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, M, K, N, bits, group_size, dtype, workspace,
                        workspace_bytes, stream);
   if (decode_supported(a)) return check_cuda(launch_decode(a), "b2q_mm(decode)");
-  // 9 <= M <= B2Q_DECODE_BLOCKS_M (default off): passes of the decode tier over blocks of 8 rows, an earlier answer to
-  // the padded 128-token tile's waste; superseded by the small-batch tier (b2q_midm.cu), kept for A/B measurements
-  {
-    MmArgs a8 = a;
-    a8.M = 8;
-    if (M > 8 && M <= env().decode_blocks_m && decode_supported(a8) && perm == nullptr) {
-      for (int m0 = 0; m0 < M; m0 += 8) {
-        MmArgs ab = a;
-        ab.M = (M - m0 < 8) ? (M - m0) : 8;
-        ab.x = static_cast<const char*>(x) + (size_t)m0 * K * 2;
-        ab.out = static_cast<char*>(out) + (size_t)m0 * N * 2;
-        int e = check_cuda(launch_decode(ab), "b2q_mm(decode x blocks)");
-        if (e != 0) return e;
-      }
-      return 0;
-    }
-  }
   if (M == 1 && bits == 8 && K % 128 == 0) return check_cuda(launch_gemv(a), "b2q_mm(gemv)");
   return check_cuda(launch_gemm(a), "b2q_mm(gemm)");
 }

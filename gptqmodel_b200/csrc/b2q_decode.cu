@@ -29,19 +29,9 @@ namespace b2q {
 template <typename T, bool ASYM, bool G64, bool MOE>
 __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     decode_kernel(const __grid_constant__ DecSets S, const int32_t* __restrict__ perm, const T* __restrict__ x, int M,
-                  int K, int gsh, int qpc, int max_tiles, int ngroups, int stl,
-                  const __grid_constant__ DecodeAR ar, unsigned long long* __restrict__ trace) {
+                  int K, int gsh, int qpc, int max_tiles, int stl, const __grid_constant__ DecodeAR ar) {
   using E = ET<T>;
   extern __shared__ __align__(128) uint8_t dsm[];
-  // optional phase timestamps (debug): trace[blockIdx.x * 16 + slot] = %globaltimer (ns)
-  auto stamp = [&](int slot) {
-    if (trace != nullptr && threadIdx.x == 0 && blockIdx.y == 0) {
-      unsigned long long tns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tns));
-      trace[blockIdx.x * 16 + slot] = tns;
-    }
-  };
-  stamp(0);
   // MoE decode (DecSets::moe): the experts are data of an earlier kernel, so nothing expert-dependent may be prefetched
   // ahead of the PDL wait — the wait moves to the top (the later one is then a no-op)
   if (MOE) asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -49,15 +39,12 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   //               part[max_tiles][8][32] | mbarriers[nwarps][DEC_STAGES]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int g = lane >> 2, t = lane & 3;
-  // The CTA's warps form `ngroups` independent groups (1 or 2); a group owns whole tiles (group-strided over the
-  // launch) and its `gw` warps split the k-quads of a tile.  With 2 groups, one group's tile epilogue (barrier + cross-
-  // warp reduction, mostly latency) overlaps the other group's main loop on the same SM.
-  const int gw = nwarps / ngroups;              // warps per group
-  const int grp = warp / gw, wg = warp - grp * gw;
-  const int C = gridDim.x * ngroups;            // tile stride of a group
-  const int tile0 = (int)blockIdx.x * ngroups + grp;
+  // The CTA walks tiles tile0, tile0 + C, ...; all `gw` warps split the k-quads of every tile (wg = warp's index).
+  const int gw = nwarps, wg = warp;
+  const int C = gridDim.x;                      // tile stride of a CTA
+  const int tile0 = (int)blockIdx.x;
   const int TT = S.tile_end[S.nsets - 1];       // tiles of all sets
-  const int ntiles = (tile0 < TT) ? (TT - tile0 + C - 1) / C : 0;  // tiles of this group
+  const int ntiles = (tile0 < TT) ? (TT - tile0 + C - 1) / C : 0;  // tiles of this CTA
   const int nquads = K >> 7;
   // moe == 2: every cluster rank owns a whole expert (k-range 0 .. K of ITS weights) and its own row of activations
   const int q0 = (MOE && S.moe >= 2) ? 0 : blockIdx.y * qpc;
@@ -69,7 +56,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   T* sx = reinterpret_cast<T*>(dsm + (size_t)nwarps * nst * DEC_QUAD_BYTES);
   float* xsum = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sx) + (size_t)M * kspan * sizeof(T));
   float* red = xsum + qpc * 2 * 8;
-  float* part = red + 2 * nwarps * 256;  // [ngroups][max_tiles][256]
+  float* part = red + 2 * nwarps * 256;  // [max_tiles][256]
   const uint32_t bars = smem_u32(part + max_tiles * 256) + warp * DEC_STAGES * 8;
   const bool PERM = perm != nullptr;
 
@@ -150,71 +137,27 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   if (PERM) prefetch_inverse_perm(perm + K, K);
   // zero the token columns >= M of the block sums once (read by the fix-up of lanes whose columns are padding): own shared
   // memory, nothing to wait for — everything between griddepcontrol.wait and the first main-loop iteration is on the critical
-  // path of every launch
-  const bool OWN = !PERM && ngroups == 1;  // per-warp staging (stage_x_own_quads): no CTA barrier before the main loop
-  if (OWN) {
+  // path of every launch.  Without act-order every warp stages its own quads (stage_x_own_quads): no CTA barrier before
+  // the main loop.
+  if (!PERM) {
     zero_own_xsum_padding(xsum, M, nq, wg, gw);
   } else {
     for (int i = threadIdx.x; i < (q1 - q0) * 2 * 8; i += blockDim.x)
       if ((i & 7) >= M) xsum[i] = 0.f;
   }
   // PDL: let the next kernel start its own weight prefetch; wait for the producer of x only now.
-  stamp(1);
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  stamp(2);
 
   // ---- 2. stage x[m, k-range] (act-order gather fused) + per-(64 k block, token) sums, ONCE ------
-  // A thread's loads (up to SX_UNROLL x 16 bytes, K = 14336 needs 3.5 per thread) are all issued BEFORE the first is
-  // consumed: a rolled loop pays one dependent L2 round trip per iteration.
   if (MOE && S.moe == 3) {
     stage_x_own_quads<T, true>(x, sx, xsum, 1, K, q0, nq, wg, gw, kspan);
-  } else if (OWN) {
+  } else if (!PERM) {
     stage_x_own_quads<T>(x, sx, xsum, M, K, q0, nq, wg, gw, kspan);
-  } else if (PERM) {
-    stage_x_act_order<T>(x, perm + K, sx, xsum, M, K, q0 * 128, (q1 - q0) * 128, kspan);
   } else {
-    const int n8 = (q1 - q0) * 16;   // uint4 (8 halves) per token row in this CTA's k-range
-    const int tot = M * n8;
-    const int totr = (tot + 31) & ~31;
-    constexpr int SX_UNROLL = 4;
-    auto f2 = [](uint32_t u) {
-      const T* h = reinterpret_cast<const T*>(&u);
-      return E::to_f(h[0]) + E::to_f(h[1]);
-    };
-    for (int i0 = threadIdx.x; i0 < totr; i0 += blockDim.x * SX_UNROLL) {
-      uint4 xv[SX_UNROLL];
-      int mm[SX_UNROLL], jj[SX_UNROLL];
-#pragma unroll
-      for (int u = 0; u < SX_UNROLL; ++u) {
-        const int i = i0 + u * blockDim.x;
-        xv[u] = make_uint4(0, 0, 0, 0);
-        mm[u] = 0;
-        jj[u] = 0;
-        if (i < tot) {
-          const int m = (M == 1) ? 0 : i / n8, j = i - m * n8;  // batch-1 decode: no integer division ahead of the load
-          mm[u] = m;
-          jj[u] = j;
-          const T* xr = x + (size_t)m * K;
-          xv[u] = reinterpret_cast<const uint4*>(xr + (size_t)q0 * 128)[j];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < SX_UNROLL; ++u) {
-        const int i = i0 + u * blockDim.x;
-        if (i < totr) {  // warp-uniform (totr and the strides are multiples of 32)
-          if (i < tot) reinterpret_cast<uint4*>(sx + (size_t)mm[u] * kspan)[jj[u]] = xv[u];
-          float sm = (f2(xv[u].x) + f2(xv[u].y)) + (f2(xv[u].z) + f2(xv[u].w));
-          sm += __shfl_xor_sync(0xffffffffu, sm, 1);
-          sm += __shfl_xor_sync(0xffffffffu, sm, 2);
-          sm += __shfl_xor_sync(0xffffffffu, sm, 4);
-          if ((i & 7) == 0 && i < tot) xsum[(jj[u] >> 3) * 8 + mm[u]] = sm;  // 8 uint4 = one 64-k block
-        }
-      }
-    }
+    stage_x_act_order<T>(x, perm + K, sx, xsum, M, K, q0 * 128, (q1 - q0) * 128, kspan);
   }
-  if (!OWN) __syncthreads();
-  stamp(3);
+  if (PERM) __syncthreads();
 
   // ---- 3. loop over this CTA's tiles; inside a tile the warps split the k-quads --------------------
   // All loop-carried addresses are 32-bit shared-window addresses / running global pointers computed ONCE here:
@@ -316,18 +259,17 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     // (decoupled variants — "last warp to arrive reduces", "rotating reducer warp on a split arrive/sync named
     //  barrier" — add synchronisation without removing the barrier's latency)
     // tot[ftl][c]: feature nt*32 + ftl*16 + g (+8 if c >= 2), token 2t + (c & 1)
-    if (ti < 5) stamp(4 + 2 * ti);
-    float* rbuf = red + (grp * 2 + (ti & 1)) * gw * 256;
+    float* rbuf = red + (ti & 1) * gw * 256;
 #pragma unroll
     for (int a = 0; a < 2; ++a)
 #pragma unroll
       for (int b = 0; b < 4; ++b) rbuf[(wg * 8 + a * 4 + b) * 32 + lane] = tot[a][b];
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(gw * 32) : "memory");  // this group's warps only
+    asm volatile("bar.sync 1, %0;" ::"r"(gw * 32) : "memory");
     for (int i = wg * 32 + lane; i < 256; i += gw * 32) {
       float v = 0.f;
       for (int w = 0; w < gw; ++w) v += rbuf[w * 256 + i];
       if (nrank > 1) {
-        part[(grp * max_tiles + ti) * 256 + i] = v;
+        part[ti * 256 + i] = v;
       } else {
         const int acc = i >> 5, ln = i & 31;
         const int m = 2 * (ln & 3) + (acc & 1);
@@ -349,9 +291,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
         }
       }
     }
-    if (ti < 5) stamp(5 + 2 * ti);
   }
-  stamp(15);
 
   // ---- 3b. fused all-reduce across GPUs (same protocol as decode2_kernel; one tile per CTA, nrank == 1) ------------
   if (ar.world > 1) {
@@ -398,7 +338,6 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     __syncthreads();  // every tile's reducer has written its partials
     cluster_sync_all();
     const uint32_t rank = cluster_ctarank();
-    // each group reduces its own tiles (same tile <-> group mapping in every rank of the cluster)
     for (int ti = (int)rank; ti < ntiles; ti += (int)nrank) {
       const TileRef<T> tr = resolve_tile<T, MOE>(S, tile0 + ti * C);
       const int nt = tr.nt, N = tr.N;
@@ -410,7 +349,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
         if (m < M) {
           float v = 0.f;
           for (uint32_t r = 0; r < nrank; ++r) {
-            float pr = ld_dsmem_f32(smem_u32(&part[(grp * max_tiles + ti) * 256 + i]), r);
+            float pr = ld_dsmem_f32(smem_u32(&part[ti * 256 + i]), r);
             // MoE down: rank r holds expert r's complete output: y_r = T(h_r W2) like the module, then the routing weight
             if (MOE && S.moe >= 2) pr = S.wts[r] * E::to_f(E::from_f(pr));
             v += pr;
@@ -426,10 +365,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   }
 }
 
-void* g_trace_ptr = nullptr;
-
 struct DecodeCfg {
-  int C, ks, warps, qpc, max_tiles, ngroups, stl;
+  int C, ks, warps, qpc, max_tiles, stl;
   size_t smem;
 };
 
@@ -444,38 +381,32 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
   const int SMS = num_sms();
   double best_cost = 1e30;
   bool found = false;
-  const bool two_groups = env().decode_groups2 != 0;
   for (int ks = 1; ks <= 8; ks *= 2) {
     if (a.tune_ks > 0 && ks != a.tune_ks) continue;
     if (ks > quads) break;
     const int qpc = (quads + ks - 1) / ks;
     for (int warps = 4; warps <= DEC_MAX_WARPS; warps *= 2) {  // 4, 8, 16
       if (a.tune_warps > 0 && warps != a.tune_warps) continue;
-      // two independent 8-warp groups per CTA overlap one group's tile epilogue with the other's main loop (+5 % on the
-      // Llama-3-8B step) but one full-size parity case failed with it in round 1: experimental, off by default
-      int ngroups = 1;
-      if (two_groups && warps == 16 && ks == 1) ngroups = 2;  // (the split-K + groups combination faults)
-      const int gwarps = warps / ngroups;
       int C = SMS / ks;
-      if (C * ngroups > NT) C = (NT + ngroups - 1) / ngroups;
+      if (C > NT) C = NT;
       if (C < 1) C = 1;
-      const int max_tiles = (NT + C * ngroups - 1) / (C * ngroups);  // per group
+      const int max_tiles = (NT + C - 1) / C;
       // ring depth 4 when it fits, else 2
       int stl = 2;
-      size_t smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles * ngroups : 0, 4);
+      size_t smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles : 0, 4);
       if (smem > 200 * 1024) {
         stl = 1;
-        smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles * ngroups : 0, 2);
+        smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles : 0, 2);
       }
       if (smem > 200 * 1024) continue;
-      const int qpw = (qpc + gwarps - 1) / gwarps;  // quads per warp per tile
+      const int qpw = (qpc + warps - 1) / warps;  // quads per warp per tile
       // relative cost in units of one quad per warp: per tile = quads/warp + barrier epilogue, split-K adds a cluster
       // barrier + DSMEM pass, fewer warps hide less latency (the weights are heuristic, not fitted to one GPU)
       const double cost =
-          (double)max_tiles * (qpw + 0.35) / ngroups + (ks > 1 ? 0.6 : 0.0) + (16 - warps) * 0.04 * max_tiles * qpw;
+          (double)max_tiles * (qpw + 0.35) + (ks > 1 ? 0.6 : 0.0) + (16 - warps) * 0.04 * max_tiles * qpw;
       if (cost < best_cost) {
         best_cost = cost;
-        best = DecodeCfg{C, ks, warps, qpc, ks > 1 ? max_tiles : 0, ngroups, stl, smem};
+        best = DecodeCfg{C, ks, warps, qpc, ks > 1 ? max_tiles : 0, stl, smem};
         found = true;
       }
     }
@@ -486,17 +417,17 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
 bool decode2_plan(const MmArgs& a, int NT, int* out8);  // b2q_decode2.cu
 
 // Host-side planner query (b2q_debug_decode_plan): {C, ks, warps, warps per group, quads per CTA, max tiles per group,
-// ring stages, dynamic shared memory bytes}
+// ring stages, dynamic shared memory bytes}; decode_kernel runs one group of all the CTA's warps
 bool decode_plan(int version, const MmArgs& a, int NT, int* out8) {
   if (version == 2) return decode2_plan(a, NT, out8);
   DecodeCfg c;
   if (!decode_config(a, NT, c)) return false;
-  const int v[8] = {c.C, c.ks, c.warps, c.warps / c.ngroups, c.qpc, c.max_tiles, 1 << c.stl, (int)c.smem};
+  const int v[8] = {c.C, c.ks, c.warps, c.warps, c.qpc, c.max_tiles, 1 << c.stl, (int)c.smem};
   for (int i = 0; i < 8; ++i) out8[i] = v[i];
   return true;
 }
 
-template <typename T, bool ASYM, bool G64, bool MOE = false>
+template <typename T, bool ASYM, bool G64, bool MOE>
 static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodeCfg& c, const DecodeAR& ar) {
   auto kern = decode_kernel<T, ASYM, G64, MOE>;
   if (c.smem > 48 * 1024) {
@@ -521,8 +452,21 @@ static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodeCfg
   if (a.group_size == 64) gsh = 0;
   else if (a.group_size == 128) gsh = 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, sets, a.perm, (const T*)a.x, a.M, a.K, gsh, c.qpc, c.max_tiles,
-                                     c.ngroups, c.stl, ar, (unsigned long long*)g_trace_ptr);
+                                     c.stl, ar);
   return (int)e;
+}
+
+// The one-token MoE launches (DecSets::moe != 0) run their own instantiation.
+static int launch_decode_cfg(const MmArgs& a, const DecSets& sets, const DecodeCfg& c, const DecodeAR& ar) {
+  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
+#define B2Q_DEC_CASE(T, MOE)                                                   \
+  (asym ? (g64 ? launch_decode_t<T, true, true, MOE>(a, sets, c, ar)           \
+               : launch_decode_t<T, true, false, MOE>(a, sets, c, ar))         \
+        : (g64 ? launch_decode_t<T, false, true, MOE>(a, sets, c, ar)          \
+               : launch_decode_t<T, false, false, MOE>(a, sets, c, ar)))
+  if (sets.moe != 0) return a.dtype == 0 ? B2Q_DEC_CASE(__half, true) : B2Q_DEC_CASE(__nv_bfloat16, true);
+  return a.dtype == 0 ? B2Q_DEC_CASE(__half, false) : B2Q_DEC_CASE(__nv_bfloat16, false);
+#undef B2Q_DEC_CASE
 }
 
 bool decode_supported(const MmArgs& a) {
@@ -530,7 +474,7 @@ bool decode_supported(const MmArgs& a) {
          (a.group_size == 64 || a.group_size == 128 || a.group_size == a.K);
 }
 
-int launch_decode2_sets(const MmArgs& a, const DecSets& sets);  // b2q_decode2.cu (experimental), -2 = no configuration
+int launch_decode2_sets(const MmArgs& a, const DecSets& sets);  // b2q_decode2.cu, -2 = no configuration
 
 static int launch_decode_sets(const MmArgs& a, const DecSets& sets) {
   // Kernel choice per launch shape: launches whose CTAs walk SEVERAL 32-feature tiles (more tiles than SMs: fused q|k|v,
@@ -558,16 +502,7 @@ static int launch_decode_sets(const MmArgs& a, const DecSets& sets) {
               a.tune_warps);
     return -1;
   }
-  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
-  const DecodeAR none = {};
-#define B2Q_DEC_CASE(T, MOE)                                                     \
-  (asym ? (g64 ? launch_decode_t<T, true, true, MOE>(a, sets, c, none)           \
-               : launch_decode_t<T, true, false, MOE>(a, sets, c, none))         \
-        : (g64 ? launch_decode_t<T, false, true, MOE>(a, sets, c, none)          \
-               : launch_decode_t<T, false, false, MOE>(a, sets, c, none)))
-  if (sets.moe != 0) return a.dtype == 0 ? B2Q_DEC_CASE(__half, true) : B2Q_DEC_CASE(__nv_bfloat16, true);
-  return a.dtype == 0 ? B2Q_DEC_CASE(__half, false) : B2Q_DEC_CASE(__nv_bfloat16, false);
-#undef B2Q_DEC_CASE
+  return launch_decode_cfg(a, sets, c, DecodeAR{});
 }
 
 // Row-parallel shard + all-reduce on decode_kernel: only for launches in which every CTA owns at most ONE tile and K is not
@@ -579,15 +514,8 @@ int launch_decode1_allreduce(const MmArgs& a, const DecSets& sets, const DecodeA
   MmArgs a1 = a;
   a1.tune_ks = 1;
   DecodeCfg c;
-  if (!decode_config(a1, NT, c) || c.ks != 1 || c.ngroups != 1 || c.C < NT || c.C > 160) return -2;
-  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
-#define B2Q_DEC_CASE(T)                                                          \
-  (asym ? (g64 ? launch_decode_t<T, true, true>(a1, sets, c, ar)                 \
-               : launch_decode_t<T, true, false>(a1, sets, c, ar))               \
-        : (g64 ? launch_decode_t<T, false, true>(a1, sets, c, ar)                \
-               : launch_decode_t<T, false, false>(a1, sets, c, ar)))
-  return a.dtype == 0 ? B2Q_DEC_CASE(__half) : B2Q_DEC_CASE(__nv_bfloat16);
-#undef B2Q_DEC_CASE
+  if (!decode_config(a1, NT, c) || c.ks != 1 || c.C < NT || c.C > 160) return -2;
+  return launch_decode_cfg(a1, sets, c, ar);
 }
 
 int launch_decode(const MmArgs& a) {
@@ -708,7 +636,6 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
   DecodeCfg c = {};
   c.ks = top_k;
   c.warps = DEC_MAX_WARPS;
-  c.ngroups = 1;
   c.qpc = a.K / 128;  // a rank's k-range is its expert's whole K
   c.C = num_sms() / top_k;
   if (c.C > NT) c.C = NT;
@@ -726,15 +653,7 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
   MmArgs a0 = a;
   a0.perm = nullptr;
   a0.bias = nullptr;
-  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
-  const DecodeAR none = {};
-#define B2Q_DEC_CASE(T)                                                            \
-  (asym ? (g64 ? launch_decode_t<T, true, true, true>(a0, sets, c, none)           \
-               : launch_decode_t<T, true, false, true>(a0, sets, c, none))         \
-        : (g64 ? launch_decode_t<T, false, true, true>(a0, sets, c, none)          \
-               : launch_decode_t<T, false, false, true>(a0, sets, c, none)))
-  return a.dtype == 0 ? B2Q_DEC_CASE(__half) : B2Q_DEC_CASE(__nv_bfloat16);
-#undef B2Q_DEC_CASE
+  return launch_decode_cfg(a0, sets, c, DecodeAR{});
 }
 
 }  // namespace b2q

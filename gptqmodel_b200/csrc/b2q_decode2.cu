@@ -4,19 +4,18 @@
 //
 // Same data path as b2q_decode.cu (fragment-major T4 tiles -> per-warp cp.async.bulk ring -> mma.sync on raw
 // bias+q operands -> per-group fp32 fix-up, cluster split-K through distributed shared memory); what changes is
-// everything AROUND the main loop, which a phase timeline of the first kernel (tools/trace_decode.py) shows to cost as
-// much as the loop itself:
+// everything AROUND the main loop:
 //  * no per-tile epilogue: a warp parks its partial sums of a finished tile in its own slice of shared memory
 //    (tokens < M only: 128 B per warp and tile at M = 1) and moves on; the CTA meets ONCE, after its last tile, and
 //    reduces all tiles together.  v1 paid a CTA barrier + a 16-partial reduction (mostly latency) per tile,
 //    3-7 times per launch;
 //  * because nothing synchronises the warps between tiles any more, the warps of a CTA can form independent groups
 //    of `gw` warps that walk different tiles (gw = 16, 8, 4 ...): the launch picks (split-K ranks, warps, gw)
-//    minimising quads per warp, so small K-slices no longer leave warps idle;
-//  * activations arrive by ONE cp.async.bulk per token row (issued right after griddepcontrol.wait) instead of a
-//    strided LDG/STS loop (3.5 dependent L2 round trips per thread at K = 14336), and every warp sums the activations
-//    of its OWN k-quads (the same quads in every tile), so no CTA barrier separates staging from the main loop.
-//    Act-order layers keep the gather loop of v1 (a gather cannot be a bulk copy).
+//    minimising quads per warp, so small K-slices no longer leave warps idle.
+// The activations are staged as in v1: with one warp group every warp stages and sums its OWN k-quads (the same quads in
+// every tile), so no CTA barrier separates staging from the main loop; several groups read the same quads, so the CTA
+// stages its k-range once; act-order layers gather through the inverse permutation.  B2Q_DECODE2_XTMA=1 (off by
+// default) instead loads each token row with one cp.async.bulk and lets every warp sum its own quads.
 // Arithmetic per output element is the same as v1 except for the summation order of the fp32 partials.
 #include "b2q_common.cuh"
 #include "b2q_decode.cuh"
@@ -26,15 +25,6 @@ namespace b2q {
 
 constexpr int DEC_AR_MAXCTA = 160;  // flag columns per source rank (>= CTAs of one launch: one per SM)
 int launch_decode1_allreduce(const MmArgs& a, const DecSets& sets, const DecodeAR& ar);  // b2q_decode.cu
-
-// Cluster barrier whose memory ordering is only CTA-scope: a cluster-scope release can compile to MEMBAR.ALL.GPU,
-// which waits on the whole memory system although the data exchanged here lives in
-// shared memory, whose single point of coherence is the owning SM.  MEMBAR.ALL.CTA makes this thread's shared-memory
-// stores (and outstanding DSMEM loads) performed before the relaxed arrive.  Weaker than the PTX model asks for:
-// selected only with B2Q_DECODE2_FASTSYNC=1 (A/B switch), default is cluster_sync_all().
-__device__ __forceinline__ void cluster_sync_cta_fenced() {
-  asm volatile("fence.acq_rel.cta;\n\tbarrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
 
 __device__ __forceinline__ void dec_st_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -62,17 +52,9 @@ template <typename T, bool ASYM, bool G64, bool MOE>
 __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     decode2_kernel(const __grid_constant__ DecSets S, const int32_t* __restrict__ perm, const T* __restrict__ x, int M,
                    int K, int gsh, int qpc, int max_tiles, int gw, int stl, int xtma,
-                   const __grid_constant__ DecodeAR ar, unsigned long long* __restrict__ trace) {
+                   const __grid_constant__ DecodeAR ar) {
   using E = ET<T>;
   extern __shared__ __align__(128) uint8_t dsm2[];
-  auto stamp = [&](int slot) {
-    if (trace != nullptr && threadIdx.x == 0 && blockIdx.y == 0) {
-      unsigned long long tns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tns));
-      trace[blockIdx.x * 16 + slot] = tns;
-    }
-  };
-  stamp(0);
   // MoE decode (DecSets::moe == 1): expert ids are data of an earlier kernel — wait before the first expert-dependent address
   if (MOE) asm volatile("griddepcontrol.wait;" ::: "memory");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -99,7 +81,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   const uint32_t bars = bars0 + warp * DEC_STAGES * 8;
   const uint32_t xbar = bars0 + nwarps * DEC_STAGES * 8;
   const bool PERM = perm != nullptr;
-  const bool XTMA = (xtma & 1) != 0 && !PERM;  // xtma bit 0: bulk-copied activations, bit 1: CTA-fenced cluster barriers
+  const bool XTMA = (xtma & 1) != 0 && !PERM;  // bulk-copied activations (B2Q_DECODE2_XTMA=1)
 
   // ---- 1. the first ring stages of this warp requested before anything else -------------------------
   const int nq = (q0 + wg < q1) ? (q1 - q0 - wg + gw - 1) / gw : 0;  // quads per tile for this warp
@@ -185,10 +167,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     for (int i = threadIdx.x; i < (q1 - q0) * 2 * 8; i += blockDim.x)
       if ((i & 7) >= M) xsum[i] = 0.f;
   }
-  stamp(1);
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  stamp(2);
 
   const uint32_t xf_a0 = smem_u32(sx) + (uint32_t)((g * kspan + t * 16 + wg * 128) * 2);
   const uint32_t xs_a0 = smem_u32(xsum) + (uint32_t)((2 * t + wg * 16) * 4);
@@ -233,7 +213,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     stage_x_act_order<T>(x, perm + K, sx, xsum, M, K, q0 * 128, (q1 - q0) * 128, kspan);
     __syncthreads();
   } else {
-    // LDG staging (B2Q_DECODE2_XTMA=0, the default): the staging loop of v1
+    // several warp groups read the same quads: the CTA stages its k-range once
     const int n8 = (q1 - q0) * 16;  // uint4 (8 halves) per token row in this CTA's k-range
     const int tot = M * n8;
     const int totr = (tot + 31) & ~31;
@@ -259,7 +239,6 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     }
     __syncthreads();
   }
-  stamp(3);
 
   // ---- 3. main loop: the warp's quads of all its tiles, no CTA-level synchronisation ------------------
   constexpr float ZSYM = 8.f;
@@ -356,7 +335,6 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
         }
       }
   }
-  stamp(4);
 
   // ---- 4. ONE meeting per CTA: warps -> CTA for all tiles, then (split-K) CTA -> cluster -----------------
   __syncthreads();
@@ -410,19 +388,16 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     if (nrank > 1) cpart[row * 32 + lane] = v;
     else emit(row, v);
   }
-  stamp(5);
   const int crank = nrank > 1 ? (int)cluster_ctarank() : 0;
   if (nrank > 1) {
-    if (xtma & 2) cluster_sync_cta_fenced();
-    else cluster_sync_all();  // every rank's cpart is complete (also a CTA barrier)
+    cluster_sync_all();  // every rank's cpart is complete (also a CTA barrier)
     for (int row = crank * nwarps + warp; row < rows; row += (int)nrank * nwarps) {
       if (!row_live(row)) continue;
       float v = 0.f;
       for (uint32_t r = 0; r < nrank; ++r) v += ld_dsmem_f32(smem_u32(&cpart[row * 32 + lane]), r);
       emit(row, v);
     }
-    if (xtma & 2) cluster_sync_cta_fenced();
-    else cluster_sync_all();  // keep every rank's smem alive until all peers have read it
+    cluster_sync_all();  // keep every rank's smem alive until all peers have read it
   }
   if (AR) {
     // ---- 5. all-reduce across GPUs over peer memory (the rows this CTA emitted are the rows it sums) ----
@@ -456,7 +431,6 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
       }
     }
   }
-  stamp(15);
 }
 
 struct Decode2Cfg {
@@ -474,13 +448,11 @@ static size_t decode2_smem(int M, int warps, int gw, int qpc, int max_tiles, int
 static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
   const int quads = a.K / 128;
   const int SMS = num_sms();
-  const int force_gw = env().decode2_gw;  // A/B switches (read once at load; b2q_debug_reload_env() re-reads them)
-  const int force_ks = env().decode2_ks;
+  const int force_gw = env().decode2_gw;  // A/B switch (read once at load; b2q_debug_reload_env() re-reads it)
   double best_cost = 1e30;
   bool found = false;
   for (int ks = 1; ks <= 8; ks *= 2) {
     if (a.tune_ks > 0 && ks != a.tune_ks) continue;
-    if (a.tune_ks <= 0 && force_ks > 0 && ks != force_ks && force_ks <= quads) continue;
     if (ks > quads) break;
     const int qpc = (quads + ks - 1) / ks;
     if ((ks - 1) * qpc >= quads) continue;  // the last rank would own no quads
@@ -550,9 +522,9 @@ static int launch_decode2_t(const MmArgs& a, const DecSets& sets, const Decode2C
   int gsh = 31;  // per-channel: every k-block is group 0
   if (a.group_size == 64) gsh = 0;
   else if (a.group_size == 128) gsh = 1;
-  const int xtma = (env().decode2_xtma ? 1 : 0) | (env().decode2_fastsync ? 2 : 0);
+  const int xtma = env().decode2_xtma ? 1 : 0;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, sets, a.perm, (const T*)a.x, a.M, a.K, gsh, c.qpc, c.max_tiles, c.gw,
-                                     c.stl, xtma, ar, (unsigned long long*)g_trace_ptr);
+                                     c.stl, xtma, ar);
   return (int)e;
 }
 

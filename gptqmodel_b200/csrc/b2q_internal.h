@@ -92,15 +92,10 @@ void set_error(const char* fmt, ...);
 struct EnvCfg {
   int disable_pdl;      // B2Q_DISABLE_PDL=1
   int midm;             // B2Q_MIDM=0           : M <= 128 on the padded 128-token prefill tile instead of b2q_midm.cu
-  int decode_blocks_m;  // B2Q_DECODE_BLOCKS_M=n: 9 <= M <= n served by passes of the decode tier over 8-row blocks (default 0)
-  int decode_groups2;   // B2Q_DECODE_GROUPS=2
   int decode_v2;        // B2Q_DECODE_V2=1 / 0  : force decode2_kernel / decode_kernel (default -1: per launch shape)
   int decode2_gw;       // B2Q_DECODE2_GW=n     : force warps per tile group of decode2_kernel
-  int decode2_ks;       // B2Q_DECODE2_KS=n     : force its split-K cluster size
   int decode2_xtma;     // B2Q_DECODE2_XTMA=1   : bulk-copied activations instead of the LDG staging loop (default 0)
-  int decode2_fastsync; // B2Q_DECODE2_FASTSYNC=1: CTA-fenced cluster barriers
   int midm_ks;          // B2Q_MIDM_KS=n        : force the split-K cluster size of the small-batch tier
-  int midm_dqg1;        // B2Q_MIDM_DQG1=1      : all dequant warps of the small-batch tier on the same k-block (debugging)
 };
 const EnvCfg& env();
 void reload_env();
@@ -120,6 +115,5 @@ inline int ensure_dyn_smem(Kern kern, int bytes, uint32_t& done_mask, const char
   if (dev < 32) done_mask |= 1u << dev;
   return 0;
 }
-extern void* g_trace_ptr;  // debug: device buffer for phase timestamps of the decode kernel (nullptr = off)
 
 }  // namespace b2q

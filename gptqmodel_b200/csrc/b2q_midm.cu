@@ -500,10 +500,6 @@ template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE 
 static int launch_midm_t(const MmArgs& a, const void* x, int ks, const MoeArgs& G = MoeArgs{}, int x_rows = 0,
                          int grid_z = 1) {
   using C = MidCfg<BITS, NTOK, PST, WST, MODE>;
-  if constexpr (BITS == 4 && MODE == 0 && DQG == MM_DQG) {
-    if (env().midm_dqg1)  // debugging: all dequant warps on the same k-block
-      return launch_midm_t<T, BITS, ASYM, NTOK, PST, WST, 0, 1>(a, x, ks, G, x_rows, grid_z);
-  }
   CUtensorMap tmap;
   if (make_x_tmap_box(&tmap, x, MODE == 0 ? a.M : x_rows, a.K, a.dtype, NTOK) != 0) return -1;
   auto kern = midm_kernel<T, BITS, ASYM, NTOK, PST, WST, MODE, DQG>;

@@ -31,12 +31,12 @@ from .adapter import Lora
 
 _DTYPE_CODE = {torch.float16: 0, torch.bfloat16: 1}
 DECODE_MAX_M = 8
-PREFILL_MIN_M = 128  # M > 128: the CTA-pair prefill tier (b2q_gemm_multi serves sibling groups there)
+PREFILL_MIN_M = 128  # M > 128: the wgmma prefill tier (b2q_gemm_multi serves sibling groups there)
 
 
 class SiblingGroup:
     """QuantLinears that consume the SAME activations (q/k/v, gate/up) served by ONE launch: `b2q_decode_multi` for
-    <= 8 tokens, `b2q_gemm_multi` (persistent prefill tier) for > 128 tokens; 9..128 tokens run per module.
+    <= 8 tokens, `b2q_gemm_multi` (wgmma prefill tier) for > 128 tokens; 9..128 tokens run per module.
 
     The first member called with a new `x` launches for all members and parks the siblings'
     outputs; each sibling's `forward(x)` then just picks its result up.  Every module keeps the reference's
@@ -89,7 +89,7 @@ class SiblingGroup:
         if M <= DECODE_MAX_M:
             check(lib.b2q_decode_multi(x2.data_ptr(), n, packed, scales, zeros, _ptr(who.perm), bias, outp, Ns, M, K,
                                        who.kbits, who._kgs, _DTYPE_CODE[x2.dtype], stream), "b2q_decode_multi")
-        else:  # prefill tier: one persistent launch over the tile columns of all siblings, x[:, perm] gathered once
+        else:  # prefill tier: one launch over the tile columns of all siblings, x[:, perm] gathered once
             ws, ws_bytes = None, 0
             if who.perm is not None:
                 ws_bytes = M * K * 2

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 4
+#define B2Q_ABI_VERSION 5
 #define B2Q_DTYPE_F16 0
 #define B2Q_DTYPE_BF16 1
 
@@ -95,8 +95,8 @@ int b2q_decode_multi(const void* x, int nsets, const void* const* packed, const 
                      const int32_t* const* qzeros, const int32_t* perm, const void* const* bias, void* const* out,
                      const int* N, int M, int K, int bits, int group_size, int dtype, void* stream);
 
-/* The same for the prefill tier (bits = 4, M > 128): the 256-feature tile columns of all sets form one index space for the
- * persistent CTA pairs (q|k|v: 192 tiles instead of 128 + 32 + 32 at M = 2048), one launch instead of nsets, and act-order
+/* The same for the prefill tier (bits = 4, M > 128): the 128-feature tile columns of all sets form one grid (q|k|v of
+ * Llama-3-8B: 48 tile columns instead of 32 + 8 + 8), one launch instead of nsets, and act-order
  * siblings gather x[:, perm] ONCE into `workspace` (>= M*K*2 bytes when perm != NULL). */
 int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const void* const* scales,
                    const int32_t* const* qzeros, const int32_t* perm, const void* const* bias, void* const* out,
@@ -188,11 +188,8 @@ size_t b2q_decode_allreduce_flag_bytes(void);
  * call path). */
 void b2q_debug_reload_env(void);
 
-/* Debug: device buffer (>= 160*16 uint64) receiving %globaltimer phase stamps of the decode kernel; NULL = off. */
-void b2q_debug_set_trace(void* device_buffer);
-
 /* Debug / tests (host only, no GPU needed): the launch plan the decode tier would use for out[M, N] with N the total
- * width of the (fused sibling) weight sets.  version 1 = b2q_decode.cu, 2 = the experimental b2q_decode2.cu.
+ * width of the (fused sibling) weight sets.  version 1 = b2q_decode.cu, 2 = b2q_decode2.cu.
  * out8 = {CTA columns, split-K ranks (cluster size), warps per CTA, warps per tile group, k-quads (128 k) per CTA,
  * tiles (32 features) per group, ring stages, dynamic shared memory bytes}.  ks / warps <= 0 = heuristic. */
 int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, int* out8);

@@ -1,4 +1,4 @@
-"""CPU model of the INDEX ARITHMETIC of the experimental decode kernel v2 (gptqmodel_b200/csrc/b2q_decode2.cu).
+"""CPU model of the INDEX ARITHMETIC of the decode kernel v2 (gptqmodel_b200/csrc/b2q_decode2.cu).
 
 The kernel cannot run without a GPU, but everything that is new in it relative to the GPU-validated v1 kernel is index
 bookkeeping: which warp walks which (tile, k-quad) units, where it parks its partial sums in shared memory, how the

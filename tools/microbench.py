@@ -174,9 +174,9 @@ def gemm(Ms=(2048,)):
 
 def midm(Ms=(9, 16, 32, 64, 128)):
     """Small-batch tier (b2q_midm.cu) per Llama-3-8B shape with weights rotated > L2: heuristic split-K vs forced cluster
-    sizes vs the round-1 paths (padded single-CTA tier; decode row blocks for M <= 16), + 8-bit and group_size 32."""
+    sizes vs the round-1 padded single-CTA tier, + 8-bit and group_size 32."""
     def setenv(**kw):
-        for k in ("B2Q_MIDM", "B2Q_MIDM_KS", "B2Q_DECODE_BLOCKS_M"):
+        for k in ("B2Q_MIDM", "B2Q_MIDM_KS"):
             os.environ.pop(k, None)
         os.environ.update({k: str(v) for k, v in kw.items()})
         g.lib.b2q_debug_reload_env()
@@ -197,8 +197,6 @@ def midm(Ms=(9, 16, 32, 64, 128)):
                 variants = [("midm", {})] + [(f"ks{k}", {"B2Q_MIDM_KS": k}) for k in (1, 2, 4, 8)]
                 if (bits, gs) == (4, 128):
                     variants.append(("padded_r1", {"B2Q_MIDM": 0}))
-                    if M <= 16:
-                        variants.append(("decode_x2_r1", {"B2Q_DECODE_BLOCKS_M": 16}))
                 for name, envs in variants:
                     setenv(**envs)
                     try:

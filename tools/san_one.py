@@ -1,10 +1,12 @@
-"""Small-shape exercise of the experimental kernels (target for compute-sanitizer; also a quick parity check).
+"""Small-shape exercise of the decode, small-batch and prefill tiers (target for compute-sanitizer; also a quick parity
+check).
 
     B2Q_DECODE_V2=1 compute-sanitizer --tool memcheck python tools/san_one.py
     ... --tool racecheck / --tool synccheck
 
-Covers: decode v2 (sym / asym g64 / act-order, M = 1, 5, 8, single set and fused siblings, forced split-K and warp groups),
-stream-K prefill (M = 300, shapes whose tile count is not a multiple of the pair count), cluster split-K (M = 40, 128).
+Covers: decode v2 (sym / asym g64 / act-order, M = 1, 5, 8, single set and fused siblings, forced warp groups), the
+small-batch tier's cluster split-K (M = 40, 128), and the prefill tier (M = 300: partial token and feature tiles) for single
+layers and fused siblings.
 """
 import os
 import sys
