@@ -87,20 +87,11 @@ int launch_allreduce(void* inout, int n, int dtype, int rank, int world, const v
                      size_t flag_offset, int max_elems, void* seq, cudaStream_t stream) {
   ARPeers p = {};
   for (int i = 0; i < world; ++i) p.buf[i] = const_cast<void*>(peer_bufs[i]);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(1, 1, 1);
-  cfg.blockDim = dim3(256, 1, 1);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = env().disable_pdl ? 0 : 1;
   if (dtype == 0)
-    return (int)cudaLaunchKernelEx(&cfg, allreduce_kernel<__half>, p, (__half*)inout, n, rank, world, max_elems,
-                                   flag_offset, (uint32_t*)seq);
-  return (int)cudaLaunchKernelEx(&cfg, allreduce_kernel<__nv_bfloat16>, p, (__nv_bfloat16*)inout, n, rank, world,
-                                 max_elems, flag_offset, (uint32_t*)seq);
+    return launch_kernel(allreduce_kernel<__half>, dim3(1, 1, 1), dim3(256, 1, 1), 0, stream, 0, true, p,
+                         (__half*)inout, n, rank, world, max_elems, flag_offset, (uint32_t*)seq);
+  return launch_kernel(allreduce_kernel<__nv_bfloat16>, dim3(1, 1, 1), dim3(256, 1, 1), 0, stream, 0, true, p,
+                       (__nv_bfloat16*)inout, n, rank, world, max_elems, flag_offset, (uint32_t*)seq);
 }
 
 }  // namespace b2q

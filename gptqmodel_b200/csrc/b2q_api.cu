@@ -129,8 +129,16 @@ static MmArgs make_args(const void* x, const void* packed, const void* scales, c
   a.stream = (cudaStream_t)stream;
   a.tune_ks = 0;
   a.tune_warps = 0;
-  a.pdl = env().disable_pdl ? 0 : 1;
   return a;
+}
+
+// forced split-K cluster size / warps per CTA of b2q_gemv and b2q_decode (0: the planner's choice)
+static int check_tune(const char* fn, int ks, int warps) {
+  if (ks > 16 || warps > 16 || (ks > 0 && (ks & (ks - 1)) != 0)) {
+    set_error("%s: ks=%d (power of two <= 16) / warps=%d (<= 16) out of range", fn, ks, warps);
+    return -2;
+  }
+  return 0;
 }
 }  // namespace b2q
 
@@ -180,8 +188,8 @@ size_t b2q_mm_workspace_bytes(int M, int K, int N, int bits, int group_size, int
   a.N = N;
   a.bits = bits;
   a.group_size = group_size;
-  if (decode_supported(a)) return 0;                 // the decode tier gathers x[perm] while staging the activations
-  if (M == 1 && bits == 8 && K % 128 == 0) return 0;  // so does the 8-bit GEMV
+  // the decode tier gathers x[perm] while staging the activations, and so does the 8-bit GEMV
+  if (decode_supported(a) || gemv_supported(a)) return 0;
   return (size_t)M * (size_t)K * 2;
 }
 
@@ -276,16 +284,14 @@ int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_
   int v = validate("b2q_gemv", x, packed, scales, out, 1, K, N, bits, group_size, dtype);
   if (v != 0) return v;
   DeviceGuard dg(packed);
-  if (ks > 16 || warps > 16 || (ks > 0 && (ks & (ks - 1)) != 0)) {
-    set_error("b2q_gemv: ks=%d (power of two <= 16) / warps=%d (<= 16) out of range", ks, warps);
-    return -2;
-  }
+  v = check_tune("b2q_gemv", ks, warps);
+  if (v != 0) return v;
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, 1, K, N, bits, group_size, dtype, nullptr, 0,
                        stream);
   a.tune_ks = ks;
   a.tune_warps = warps;
   if (decode_supported(a)) return check_cuda(launch_decode(a), "b2q_gemv(decode)");
-  if (bits == 8 && K % 128 == 0) return check_cuda(launch_gemv(a), "b2q_gemv");
+  if (gemv_supported(a)) return check_cuda(launch_gemv(a), "b2q_gemv");
   set_error("b2q_gemv: no M=1 tier for bits=%d K=%d group_size=%d (use b2q_mm)", bits, K, group_size);
   return -2;
 }
@@ -296,10 +302,8 @@ int b2q_decode(const void* x, const void* packed, const void* scales, const int3
   int v = validate("b2q_decode", x, packed, scales, out, M, K, N, bits, group_size, dtype);
   if (v != 0) return v;
   DeviceGuard dg(packed);
-  if (ks > 16 || warps > 16 || (ks > 0 && (ks & (ks - 1)) != 0)) {
-    set_error("b2q_decode: ks=%d (power of two <= 16) / warps=%d (<= 16) out of range", ks, warps);
-    return -2;
-  }
+  v = check_tune("b2q_decode", ks, warps);
+  if (v != 0) return v;
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, M, K, N, bits, group_size, dtype, nullptr, 0,
                        stream);
   a.tune_ks = ks;
@@ -382,7 +386,7 @@ int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t*
   MmArgs a = make_args(x, packed, scales, qzeros, perm, bias, out, M, K, N, bits, group_size, dtype, workspace,
                        workspace_bytes, stream);
   if (decode_supported(a)) return check_cuda(launch_decode(a), "b2q_mm(decode)");
-  if (M == 1 && bits == 8 && K % 128 == 0) return check_cuda(launch_gemv(a), "b2q_mm(gemv)");
+  if (gemv_supported(a)) return check_cuda(launch_gemv(a), "b2q_mm(gemv)");
   return check_cuda(launch_gemm(a), "b2q_mm(gemm)");
 }
 

@@ -365,18 +365,13 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   }
 }
 
-struct DecodeCfg {
-  int C, ks, warps, qpc, max_tiles, stl;
-  size_t smem;
-};
-
 static size_t decode_smem(int M, int warps, int qpc, int max_tiles, int nst) {
   return (size_t)warps * nst * DEC_QUAD_BYTES + (size_t)M * qpc * 128 * 2 + (size_t)qpc * 2 * 8 * 4 +
          (size_t)2 * warps * 256 * 4 + (size_t)max_tiles * 256 * 4 + (size_t)warps * DEC_STAGES * 8 + 16;
 }
 
 // Pick (C tile-columns, ks split-K ranks, warps) minimising the critical path in "quads per warp" on one CTA per SM.
-static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
+static bool decode_config(const MmArgs& a, int NT, DecodePlan& best) {
   const int quads = a.K / 128;
   const int SMS = num_sms();
   double best_cost = 1e30;
@@ -391,14 +386,8 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
       if (C > NT) C = NT;
       if (C < 1) C = 1;
       const int max_tiles = (NT + C - 1) / C;
-      // ring depth 4 when it fits, else 2
-      int stl = 2;
-      size_t smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles : 0, 4);
-      if (smem > 200 * 1024) {
-        stl = 1;
-        smem = decode_smem(a.M, warps, qpc, ks > 1 ? max_tiles : 0, 2);
-      }
-      if (smem > 200 * 1024) continue;
+      DecodePlan p = {C, ks, warps, warps, qpc, ks > 1 ? max_tiles : 0, 0, 0};
+      if (!fit_ring(p, [&](int nst) { return decode_smem(a.M, warps, qpc, p.max_tiles, nst); })) continue;
       const int qpw = (qpc + warps - 1) / warps;  // quads per warp per tile
       // relative cost in units of one quad per warp: per tile = quads/warp + barrier epilogue, split-K adds a cluster
       // barrier + DSMEM pass, fewer warps hide less latency (the weights are heuristic, not fitted to one GPU)
@@ -406,7 +395,7 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
           (double)max_tiles * (qpw + 0.35) + (ks > 1 ? 0.6 : 0.0) + (16 - warps) * 0.04 * max_tiles * qpw;
       if (cost < best_cost) {
         best_cost = cost;
-        best = DecodeCfg{C, ks, warps, qpc, ks > 1 ? max_tiles : 0, stl, smem};
+        best = p;
         found = true;
       }
     }
@@ -414,59 +403,28 @@ static bool decode_config(const MmArgs& a, int NT, DecodeCfg& best) {
   return found;
 }
 
-bool decode2_plan(const MmArgs& a, int NT, int* out8);  // b2q_decode2.cu
-
 // Host-side planner query (b2q_debug_decode_plan): {C, ks, warps, warps per group, quads per CTA, max tiles per group,
-// ring stages, dynamic shared memory bytes}; decode_kernel runs one group of all the CTA's warps
+// ring stages, dynamic shared memory bytes}
 bool decode_plan(int version, const MmArgs& a, int NT, int* out8) {
-  if (version == 2) return decode2_plan(a, NT, out8);
-  DecodeCfg c;
-  if (!decode_config(a, NT, c)) return false;
-  const int v[8] = {c.C, c.ks, c.warps, c.warps, c.qpc, c.max_tiles, 1 << c.stl, (int)c.smem};
+  DecodePlan c;
+  if (!(version == 2 ? decode2_config(a, NT, c) : decode_config(a, NT, c))) return false;
+  const int v[8] = {c.C, c.ks, c.warps, c.gw, c.qpc, c.max_tiles, 1 << c.stl, (int)c.smem};
   for (int i = 0; i < 8; ++i) out8[i] = v[i];
   return true;
 }
 
-template <typename T, bool ASYM, bool G64, bool MOE>
-static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodeCfg& c, const DecodeAR& ar) {
-  auto kern = decode_kernel<T, ASYM, G64, MOE>;
-  if (c.smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem);
-    if (e != cudaSuccess) return (int)e;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(c.C, c.ks, 1);
-  cfg.blockDim = dim3(c.warps * 32, 1, 1);
-  cfg.dynamicSmemBytes = c.smem;
-  cfg.stream = a.stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1;
-  attr[0].val.clusterDim.y = c.ks;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = a.pdl ? 2 : 1;
-  int gsh = 31;  // per-channel: every k-block is group 0
-  if (a.group_size == 64) gsh = 0;
-  else if (a.group_size == 128) gsh = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, sets, a.perm, (const T*)a.x, a.M, a.K, gsh, c.qpc, c.max_tiles,
-                                     c.stl, ar);
-  return (int)e;
+template <typename I>
+static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodePlan& c, const DecodeAR& ar) {
+  using T = typename I::T;
+  auto kern = decode_kernel<T, I::ASYM, I::G64, I::MOE>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, (int)c.smem, smem_opted, "b2q_decode")) return e;
+  return launch_kernel(kern, dim3(c.C, c.ks, 1), dim3(c.warps * 32, 1, 1), c.smem, a.stream, c.ks, true, sets, a.perm,
+                       (const T*)a.x, a.M, a.K, decode_gsh(a.group_size), c.qpc, c.max_tiles, c.stl, ar);
 }
 
-// The one-token MoE launches (DecSets::moe != 0) run their own instantiation.
-static int launch_decode_cfg(const MmArgs& a, const DecSets& sets, const DecodeCfg& c, const DecodeAR& ar) {
-  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
-#define B2Q_DEC_CASE(T, MOE)                                                   \
-  (asym ? (g64 ? launch_decode_t<T, true, true, MOE>(a, sets, c, ar)           \
-               : launch_decode_t<T, true, false, MOE>(a, sets, c, ar))         \
-        : (g64 ? launch_decode_t<T, false, true, MOE>(a, sets, c, ar)          \
-               : launch_decode_t<T, false, false, MOE>(a, sets, c, ar)))
-  if (sets.moe != 0) return a.dtype == 0 ? B2Q_DEC_CASE(__half, true) : B2Q_DEC_CASE(__nv_bfloat16, true);
-  return a.dtype == 0 ? B2Q_DEC_CASE(__half, false) : B2Q_DEC_CASE(__nv_bfloat16, false);
-#undef B2Q_DEC_CASE
+static int launch_decode_plan(const MmArgs& a, const DecSets& sets, const DecodePlan& c, const DecodeAR& ar) {
+  return dispatch_decode(a, sets, [&](auto inst) { return launch_decode_t<decltype(inst)>(a, sets, c, ar); });
 }
 
 bool decode_supported(const MmArgs& a) {
@@ -496,13 +454,13 @@ static int launch_decode_sets(const MmArgs& a, const DecSets& sets) {
       if (rc != -2) return rc;
     }
   }
-  DecodeCfg c;
+  DecodePlan c;
   if (!decode_config(a, sets.tile_end[sets.nsets - 1], c)) {
     set_error("b2q_decode: no configuration fits shared memory for M=%d K=%d (ks=%d warps=%d)", a.M, a.K, a.tune_ks,
               a.tune_warps);
     return -1;
   }
-  return launch_decode_cfg(a, sets, c, DecodeAR{});
+  return launch_decode_plan(a, sets, c, DecodeAR{});
 }
 
 // Row-parallel shard + all-reduce on decode_kernel: only for launches in which every CTA owns at most ONE tile and K is not
@@ -513,9 +471,9 @@ int launch_decode1_allreduce(const MmArgs& a, const DecSets& sets, const DecodeA
   if (NT > num_sms() || a.perm != nullptr) return -2;
   MmArgs a1 = a;
   a1.tune_ks = 1;
-  DecodeCfg c;
+  DecodePlan c;
   if (!decode_config(a1, NT, c) || c.ks != 1 || c.C < NT || c.C > 160) return -2;
-  return launch_decode_cfg(a1, sets, c, ar);
+  return launch_decode_plan(a1, sets, c, ar);
 }
 
 int launch_decode(const MmArgs& a) {
@@ -523,16 +481,7 @@ int launch_decode(const MmArgs& a) {
     set_error("b2q_decode: unsupported (bits=%d M=%d K=%d N=%d group=%d)", a.bits, a.M, a.K, a.N, a.group_size);
     return -1;
   }
-  DecSets sets = {};
-  sets.nsets = 1;
-  sets.tile_end[0] = a.N / 32;
-  sets.N[0] = a.N;
-  sets.packed[0] = (const uint4*)a.packed;
-  sets.scales[0] = a.scales;
-  sets.qzeros[0] = (const uint32_t*)a.qzeros;
-  sets.bias[0] = a.bias;
-  sets.out[0] = a.out;
-  return launch_decode_sets(a, sets);
+  return launch_decode_sets(a, layer_sets(a));
 }
 
 // Sibling QuantLinears (same x, same K / group size / symmetry, no act-order) in ONE launch.
@@ -619,41 +568,28 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
               "g=%d top_k=%d)", a.M, a.K, a.N, a.group_size, top_k);
     return -1;
   }
-  DecSets sets = {};
-  sets.nsets = 1;
-  const int NT = a.N / 32;
-  for (int i = 0; i < DEC_MAX_SETS; ++i) sets.tile_end[i] = NT;
-  sets.N[0] = a.N;
-  sets.packed[0] = (const uint4*)a.packed;
-  sets.scales[0] = a.scales;
-  sets.qzeros[0] = (const uint32_t*)a.qzeros;
-  sets.out[0] = a.out;
+  MmArgs a0 = a;
+  a0.perm = nullptr;
+  a0.bias = nullptr;
+  DecSets sets = layer_sets(a0);
   sets.moe = fused_act ? 3 : 2;
   sets.nexperts = E;
   sets.ids = ids;
   sets.wts = wts;
   moe_strides(sets, a.K, a.N, a.group_size);
-  DecodeCfg c = {};
+  const int NT = a.N / 32;
+  DecodePlan c = {};
   c.ks = top_k;
-  c.warps = DEC_MAX_WARPS;
+  c.warps = c.gw = DEC_MAX_WARPS;
   c.qpc = a.K / 128;  // a rank's k-range is its expert's whole K
   c.C = num_sms() / top_k;
   if (c.C > NT) c.C = NT;
   c.max_tiles = (NT + c.C - 1) / c.C;
-  c.stl = 2;
-  c.smem = decode_smem(1, c.warps, c.qpc, c.max_tiles, 4);
-  if (c.smem > 200 * 1024) {
-    c.stl = 1;
-    c.smem = decode_smem(1, c.warps, c.qpc, c.max_tiles, 2);
-  }
-  if (c.smem > 200 * 1024) {
+  if (!fit_ring(c, [&](int nst) { return decode_smem(1, c.warps, c.qpc, c.max_tiles, nst); })) {
     set_error("b2q_moe_decode_down: K=%d does not fit shared memory", a.K);
     return -1;
   }
-  MmArgs a0 = a;
-  a0.perm = nullptr;
-  a0.bias = nullptr;
-  return launch_decode_cfg(a0, sets, c, DecodeAR{});
+  return launch_decode_plan(a0, sets, c, DecodeAR{});
 }
 
 }  // namespace b2q

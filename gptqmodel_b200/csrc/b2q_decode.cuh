@@ -1,8 +1,9 @@
 // b2q_decode.cuh — definitions shared by the decode-tier kernels (b2q_decode.cu, b2q_decode2.cu): the per-warp
 // cp.async.bulk ring geometry, the mma.sync wrapper, the per-unit scale / zero registers and the multi-set ("sibling"
-// QuantLinears) tile index space.
+// QuantLinears) tile index space; on the host, the launch plan and the kernel dispatch of both.
 #pragma once
 #include "b2q_common.cuh"
+#include "b2q_internal.h"
 
 namespace b2q {
 
@@ -310,6 +311,67 @@ __device__ __forceinline__ TileRef<T> resolve_tile(const DecSets& S, int gt) {
   r.N = S.N[s];
   r.nt = gt - start;
   return r;
+}
+
+// ---- host side ---------------------------------------------------------------------------------------------------------
+// The DecSets of one QuantLinear: a's weights, bias and output.
+inline DecSets layer_sets(const MmArgs& a) {
+  DecSets s = {};
+  s.nsets = 1;
+  for (int i = 0; i < DEC_MAX_SETS; ++i) s.tile_end[i] = a.N / 32;
+  s.N[0] = a.N;
+  s.packed[0] = (const uint4*)a.packed;
+  s.scales[0] = a.scales;
+  s.qzeros[0] = (const uint32_t*)a.qzeros;
+  s.bias[0] = a.bias;
+  s.out[0] = a.out;
+  return s;
+}
+
+// Launch plan of both decode kernels: grid (C tile columns, ks split-K ranks), CTAs of `warps` warps in groups of `gw`
+// (decode_kernel: one group, gw = warps), qpc k-quads per rank, max_tiles tiles per group (0: decode_kernel without
+// split-K), 1 << stl ring stages per warp, smem bytes of dynamic shared memory.
+struct DecodePlan {
+  int C, ks, warps, gw, qpc, max_tiles, stl;
+  size_t smem;
+};
+
+// Ring depth: 4 stages when the plan fits in 200 KB of shared memory, else 2; false when neither fits.
+// smem_of(stages) is the plan's dynamic shared memory at that depth.
+template <typename SmemOf>
+inline bool fit_ring(DecodePlan& p, SmemOf smem_of) {
+  p.stl = 2;
+  p.smem = smem_of(4);
+  if (p.smem > 200 * 1024) {
+    p.stl = 1;
+    p.smem = smem_of(2);
+  }
+  return p.smem <= 200 * 1024;
+}
+
+bool decode2_config(const MmArgs& a, int NT, DecodePlan& best);  // b2q_decode2.cu
+
+// log2(64-k blocks per quantisation group) of the decode kernels; 31 = per-channel (every k-block is group 0)
+inline int decode_gsh(int group_size) { return group_size == 64 ? 0 : group_size == 128 ? 1 : 31; }
+
+// One instantiation of a decode kernel: element type, asymmetric zero points, 64-wide groups (else 128 or per-channel),
+// one-token MoE launch (DecSets::moe != 0).
+template <typename T_, bool ASYM_, bool G64_, bool MOE_>
+struct DecInst {
+  using T = T_;
+  static constexpr bool ASYM = ASYM_, G64 = G64_, MOE = MOE_;
+};
+
+// Calls launch(DecInst<...>{}) with the instantiation that serves a and sets.
+template <typename F>
+inline int dispatch_decode(const MmArgs& a, const DecSets& sets, F&& launch) {
+  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
+#define B2Q_DEC_CASE(T, MOE)                                                                      \
+  (asym ? (g64 ? launch(DecInst<T, true, true, MOE>{}) : launch(DecInst<T, true, false, MOE>{})) \
+        : (g64 ? launch(DecInst<T, false, true, MOE>{}) : launch(DecInst<T, false, false, MOE>{})))
+  if (sets.moe != 0) return a.dtype == 0 ? B2Q_DEC_CASE(__half, true) : B2Q_DEC_CASE(__nv_bfloat16, true);
+  return a.dtype == 0 ? B2Q_DEC_CASE(__half, false) : B2Q_DEC_CASE(__nv_bfloat16, false);
+#undef B2Q_DEC_CASE
 }
 
 }  // namespace b2q

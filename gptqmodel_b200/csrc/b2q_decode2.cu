@@ -433,11 +433,6 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   }
 }
 
-struct Decode2Cfg {
-  int C, ks, warps, gw, qpc, max_tiles, stl;
-  size_t smem;
-};
-
 static size_t decode2_smem(int M, int warps, int gw, int qpc, int max_tiles, int ks, int nst) {
   const size_t rows = (size_t)(warps / gw) * max_tiles * M;
   return (size_t)warps * nst * DEC_QUAD_BYTES + (size_t)M * qpc * 128 * 2 + (size_t)qpc * 2 * 8 * 4 +
@@ -445,7 +440,7 @@ static size_t decode2_smem(int M, int warps, int gw, int qpc, int max_tiles, int
 }
 
 // Pick (split-K ranks, warps per CTA, warps per group) minimising the critical path in quads per warp.
-static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
+bool decode2_config(const MmArgs& a, int NT, DecodePlan& best) {
   const int quads = a.K / 128;
   const int SMS = num_sms();
   const int force_gw = env().decode2_gw;  // A/B switch (read once at load; b2q_debug_reload_env() re-reads it)
@@ -466,13 +461,8 @@ static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
         if (C * ngroups > NT) C = (NT + ngroups - 1) / ngroups;
         if (C < 1) C = 1;
         const int max_tiles = (NT + C * ngroups - 1) / (C * ngroups);  // per group
-        int stl = 2;
-        size_t smem = decode2_smem(a.M, warps, gw, qpc, max_tiles, ks, 4);
-        if (smem > 200 * 1024) {
-          stl = 1;
-          smem = decode2_smem(a.M, warps, gw, qpc, max_tiles, ks, 2);
-        }
-        if (smem > 200 * 1024) continue;
+        DecodePlan p = {C, ks, warps, gw, qpc, max_tiles, 0, 0};
+        if (!fit_ring(p, [&](int nst) { return decode2_smem(a.M, warps, gw, qpc, max_tiles, ks, nst); })) continue;
         const int qpw = (qpc + gw - 1) / gw;  // quads per warp per tile
         const double units = (double)max_tiles * qpw;
         // relative cost in units of one quad per warp at 16 warps / SM (heuristic weights); fewer warps hide less
@@ -481,7 +471,7 @@ static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
                             0.02 * ngroups;
         if (cost < best_cost) {
           best_cost = cost;
-          best = Decode2Cfg{C, ks, warps, gw, qpc, max_tiles, stl, smem};
+          best = p;
           found = true;
         }
       }
@@ -490,58 +480,23 @@ static bool decode2_config(const MmArgs& a, int NT, Decode2Cfg& best) {
   return found;
 }
 
-bool decode2_plan(const MmArgs& a, int NT, int* out8) {
-  Decode2Cfg c;
-  if (!decode2_config(a, NT, c)) return false;
-  const int v[8] = {c.C, c.ks, c.warps, c.gw, c.qpc, c.max_tiles, 1 << c.stl, (int)c.smem};
-  for (int i = 0; i < 8; ++i) out8[i] = v[i];
-  return true;
-}
-
-template <typename T, bool ASYM, bool G64, bool MOE = false>
-static int launch_decode2_t(const MmArgs& a, const DecSets& sets, const Decode2Cfg& c, const DecodeAR& ar) {
-  auto kern = decode2_kernel<T, ASYM, G64, MOE>;
-  if (c.smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem);
-    if (e != cudaSuccess) return (int)e;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(c.C, c.ks, 1);
-  cfg.blockDim = dim3(c.warps * 32, 1, 1);
-  cfg.dynamicSmemBytes = c.smem;
-  cfg.stream = a.stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1;
-  attr[0].val.clusterDim.y = c.ks;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = a.pdl ? 2 : 1;
-  int gsh = 31;  // per-channel: every k-block is group 0
-  if (a.group_size == 64) gsh = 0;
-  else if (a.group_size == 128) gsh = 1;
+template <typename I>
+static int launch_decode2_t(const MmArgs& a, const DecSets& sets, const DecodePlan& c, const DecodeAR& ar) {
+  using T = typename I::T;
+  auto kern = decode2_kernel<T, I::ASYM, I::G64, I::MOE>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, (int)c.smem, smem_opted, "b2q_decode2")) return e;
   const int xtma = env().decode2_xtma ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, sets, a.perm, (const T*)a.x, a.M, a.K, gsh, c.qpc, c.max_tiles, c.gw,
-                                     c.stl, xtma, ar);
-  return (int)e;
+  return launch_kernel(kern, dim3(c.C, c.ks, 1), dim3(c.warps * 32, 1, 1), c.smem, a.stream, c.ks, true, sets, a.perm,
+                       (const T*)a.x, a.M, a.K, decode_gsh(a.group_size), c.qpc, c.max_tiles, c.gw, c.stl, xtma, ar);
 }
 
 // Returns -2 when no v2 configuration fits shared memory (the caller falls back to the v1 kernel).
 static int launch_decode2_ar(const MmArgs& a, const DecSets& sets, const DecodeAR& ar) {
-  Decode2Cfg c;
+  DecodePlan c;
   if (!decode2_config(a, sets.tile_end[sets.nsets - 1], c)) return -2;
   if (ar.world > 1 && c.C * c.ks > DEC_AR_MAXCTA) return -2;
-  const bool asym = a.qzeros != nullptr, g64 = a.group_size == 64;
-#define B2Q_DEC2_CASE(T, MOE)                                                          \
-  (asym ? (g64 ? launch_decode2_t<T, true, true, MOE>(a, sets, c, ar)                      \
-               : launch_decode2_t<T, true, false, MOE>(a, sets, c, ar))                    \
-        : (g64 ? launch_decode2_t<T, false, true, MOE>(a, sets, c, ar)                     \
-               : launch_decode2_t<T, false, false, MOE>(a, sets, c, ar)))
-  if (sets.moe != 0) return a.dtype == 0 ? B2Q_DEC2_CASE(__half, true) : B2Q_DEC2_CASE(__nv_bfloat16, true);
-  return a.dtype == 0 ? B2Q_DEC2_CASE(__half, false) : B2Q_DEC2_CASE(__nv_bfloat16, false);
-#undef B2Q_DEC2_CASE
+  return dispatch_decode(a, sets, [&](auto inst) { return launch_decode2_t<decltype(inst)>(a, sets, c, ar); });
 }
 
 int launch_decode2_sets(const MmArgs& a, const DecSets& sets) {
@@ -553,16 +508,7 @@ size_t decode_allreduce_flag_bytes() { return (size_t)8 * DEC_AR_MAXCTA * sizeof
 
 // Row-parallel QuantLinear shard + all-reduce(sum) across ranks in one launch (always the v2 kernel).
 int launch_decode_allreduce(const MmArgs& a, const DecodeAR& ar) {
-  DecSets sets = {};
-  sets.nsets = 1;
-  sets.tile_end[0] = a.N / 32;
-  for (int i = 1; i < DEC_MAX_SETS; ++i) sets.tile_end[i] = a.N / 32;
-  sets.N[0] = a.N;
-  sets.packed[0] = (const uint4*)a.packed;
-  sets.scales[0] = a.scales;
-  sets.qzeros[0] = (const uint32_t*)a.qzeros;
-  sets.bias[0] = a.bias;
-  sets.out[0] = a.out;
+  const DecSets sets = layer_sets(a);
   // single-tile launches run faster on decode_kernel (b2q_decode.cu), which carries the same epilogue for that case
   if (env().decode_v2 != 1) {
     const int rc1 = launch_decode1_allreduce(a, sets, ar);

@@ -342,8 +342,8 @@ static int launch_gemm_t(const MmArgs& a, const void* x, const GemmSets& S) {
   CUtensorMap tmap;
   if (make_x_tmap(&tmap, x, a.M, a.K, a.dtype) != 0) return -1;
   auto kern = gemm_kernel<T, BITS, ASYM, STAGES>;
-  static uint32_t smem_ok = 0;
-  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_ok, "b2q_gemm")) return e;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_gemm")) return e;
   dim3 grid(S.tn_end[S.nsets - 1], (a.M + G_BM - 1) / G_BM, 1);
   kern<<<grid, G_THREADS, C::SMEM_BYTES, a.stream>>>(tmap, S, a.M, a.K, gemm_gshc(a));
   return (int)cudaGetLastError();

@@ -230,29 +230,15 @@ __global__ void __launch_bounds__(GEMV_MAX_WARPS * 32)
 
 template <typename T, int BITS, bool ASYM, bool PERM>
 static int launch_gemv_t(const MmArgs& a, int ks, int warps, int cpc) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.N / 32, ks, 1);
-  cfg.blockDim = dim3(warps * 32, 1, 1);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = a.stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1;
-  attr[0].val.clusterDim.y = ks;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // PDL, see the kernel prologue
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = a.pdl ? 2 : 1;
   auto kern = gemv_kernel<T, BITS, ASYM, PERM>;
   if (ks > 8) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return (int)e;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, (const uint4*)a.packed, (const T*)a.scales,
-                                     (const uint32_t*)a.qzeros, a.perm, (const T*)a.x, (const T*)a.bias, (T*)a.out,
-                                     a.K, a.N, a.group_size, cpc);
-  return (int)e;
+  // PDL: see the kernel prologue
+  return launch_kernel(kern, dim3(a.N / 32, ks, 1), dim3(warps * 32, 1, 1), 0, a.stream, ks, true,
+                       (const uint4*)a.packed, (const T*)a.scales, (const uint32_t*)a.qzeros, a.perm, (const T*)a.x,
+                       (const T*)a.bias, (T*)a.out, a.K, a.N, a.group_size, cpc);
 }
 
 // split-K / CTA-shape heuristic: aim for >= ~4 CTAs per SM in a single wave, whole quads per warp.
@@ -270,6 +256,10 @@ static void gemv_config(const MmArgs& a, int& ks, int& warps, int& cpc) {
   while (4 * ((quads + ks - 1) / ks) > GEMV_MAX_CPC && ks < 16) ks *= 2;
   cpc = 4 * ((quads + ks - 1) / ks);
 }
+
+// The M=1 tier of 8-bit layers (b2q_mm, b2q_gemv); it gathers act-order activations itself, so b2q_mm_workspace_bytes
+// asks no workspace for it.
+bool gemv_supported(const MmArgs& a) { return a.M == 1 && a.bits == 8 && a.K % 128 == 0; }
 
 int launch_gemv(const MmArgs& a) {
   if (a.bits != 8) {

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <utility>
+
 namespace b2q {
 
 // SMs of the current device (multiProcessorCount, read once per device; an H100 SXM has 132, a PCIe card 114).  Launch plans
@@ -24,9 +26,8 @@ struct MmArgs {
   void* workspace;
   size_t workspace_bytes;
   cudaStream_t stream;
-  int tune_ks;     // >0: force GEMV cluster size (split-K)
-  int tune_warps;  // >0: force GEMV warps per CTA
-  int pdl;         // 1: launch with programmatic stream serialization (default)
+  int tune_ks;     // >0: force the split-K cluster size of the M=1 GEMV and of the decode planners
+  int tune_warps;  // >0: force the warps per CTA of the M=1 GEMV and of the decode planners
 };
 
 // Fused row-parallel all-reduce of the decode tier (b2q_decode2.cu).  world <= 1: plain decode.
@@ -43,6 +44,7 @@ size_t decode_allreduce_flag_bytes();
 int launch_prepack(const void* qweight, const int32_t* perm, void* out, int K, int N, int bits, cudaStream_t stream);
 int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
+bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier
 bool decode_supported(const MmArgs& a);
 bool decode_plan(int version, const MmArgs& a, int NT, int* out8);  // launch plan of the decode tier (host only)
@@ -101,19 +103,53 @@ const EnvCfg& env();
 void reload_env();
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: remember it per device (a process may drive
-// several GPUs, ADVICE r01), not once per process.
+// several GPUs, ADVICE r01), not once per process.  `opted[dev]` is the largest size this kernel has opted in to on
+// device dev, so a kernel whose size varies by launch plan calls the driver only when a plan needs more than before.
+// The kernels have no static shared memory, so up to 48 KB need no opt-in.
 template <typename Kern>
-inline int ensure_dyn_smem(Kern kern, int bytes, uint32_t& done_mask, const char* who) {
+inline int ensure_dyn_smem(Kern kern, int bytes, int (&opted)[32], const char* who) {
+  if (bytes <= 48 * 1024) return 0;
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 32 && ((done_mask >> dev) & 1u)) return 0;
+  if (dev < 32 && bytes <= opted[dev]) return 0;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) {
     set_error("%s: cannot opt in to %d bytes of shared memory: %s", who, bytes, cudaGetErrorString(e));
     return (int)e;
   }
-  if (dev < 32) done_mask |= 1u << dev;
+  if (dev < 32) opted[dev] = bytes;
   return 0;
+}
+
+// cudaLaunchKernelEx with the two launch attributes the project uses:
+//  * cluster_y > 0: thread-block clusters of (1, cluster_y, 1) CTAs (the split-K ranks of one tile column);
+//  * pdl: programmatic dependent launch, unless B2Q_DISABLE_PDL is set.  Only kernels that execute griddepcontrol.wait
+//    before they read their predecessor's output may be launched with it.
+template <typename... KArgs, typename... Args>
+inline int launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, int cluster_y,
+                         bool pdl, Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  unsigned n = 0;
+  if (cluster_y > 0) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = 1;
+    attr[n].val.clusterDim.y = cluster_y;
+    attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (pdl && !env().disable_pdl) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n;
+  return (int)cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
 }  // namespace b2q

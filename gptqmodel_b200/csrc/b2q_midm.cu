@@ -503,27 +503,13 @@ static int launch_midm_t(const MmArgs& a, const void* x, int ks, const MoeArgs& 
   CUtensorMap tmap;
   if (make_x_tmap_box(&tmap, x, MODE == 0 ? a.M : x_rows, a.K, a.dtype, NTOK) != 0) return -1;
   auto kern = midm_kernel<T, BITS, ASYM, NTOK, PST, WST, MODE, DQG>;
-  static uint32_t smem_ok = 0;  // per-device bit mask (a process may drive several GPUs)
-  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_ok, "b2q_midm")) return e;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_midm")) return e;
   const int nkb = a.K / MM_BK;
   const int kpc = (nkb + ks - 1) / ks;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((a.N + MM_BF - 1) / MM_BF, ks, grid_z);
-  cfg.blockDim = dim3(MM_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = a.stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1;
-  attr[0].val.clusterDim.y = ks;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = a.pdl ? 2 : 1;
-  return (int)cudaLaunchKernelEx(&cfg, kern, tmap, (const uint4*)a.packed, (const T*)a.scales,
-                                 (const uint32_t*)a.qzeros, (const T*)a.bias, (T*)a.out, a.M, a.K, a.N, gemm_gshc(a),
-                                 kpc, G);
+  return launch_kernel(kern, dim3((a.N + MM_BF - 1) / MM_BF, ks, grid_z), dim3(MM_THREADS, 1, 1), C::SMEM_BYTES,
+                       a.stream, ks, true, tmap, (const uint4*)a.packed, (const T*)a.scales, (const uint32_t*)a.qzeros,
+                       (const T*)a.bias, (T*)a.out, a.M, a.K, a.N, gemm_gshc(a), kpc, G);
 }
 
 bool midm_supported(const MmArgs& a) { return a.M >= 1 && a.M <= 128 && a.K % MM_BK == 0 && a.N % 32 == 0; }

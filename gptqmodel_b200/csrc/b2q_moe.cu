@@ -185,19 +185,12 @@ __global__ void __launch_bounds__(256)
 }
 
 int launch_moe_decode_act(const void* gu, void* h, int top_k, int N, int dtype, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((N / 2 + 255) / 256, top_k, 1);
-  cfg.blockDim = dim3(256, 1, 1);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = env().disable_pdl ? 0 : 1;
+  const dim3 grid((N / 2 + 255) / 256, top_k, 1), block(256, 1, 1);
   if (dtype == 0)
-    return (int)cudaLaunchKernelEx(&cfg, moe_decode_act_kernel<__half>, (const __half*)gu, (__half*)h, top_k, N);
-  return (int)cudaLaunchKernelEx(&cfg, moe_decode_act_kernel<__nv_bfloat16>, (const __nv_bfloat16*)gu, (__nv_bfloat16*)h,
-                                 top_k, N);
+    return launch_kernel(moe_decode_act_kernel<__half>, grid, block, 0, stream, 0, true, (const __half*)gu, (__half*)h,
+                         top_k, N);
+  return launch_kernel(moe_decode_act_kernel<__nv_bfloat16>, grid, block, 0, stream, 0, true, (const __nv_bfloat16*)gu,
+                       (__nv_bfloat16*)h, top_k, N);
 }
 
 }  // namespace b2q

@@ -142,19 +142,9 @@ __global__ void permute_cols_kernel(const uint16_t* __restrict__ x, const int32_
 
 template <int UNITS>
 static int launch_permute_rows(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream) {
-  auto kern = permute_rows_kernel<UNITS>;
   const size_t smem = (size_t)K * 2;  // <= 32 KB: inside the default dynamic shared memory limit
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(M < num_sms() * 8 ? M : num_sms() * 8, 1, 1);
-  cfg.blockDim = dim3(256, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = env().disable_pdl ? 0 : 1;
-  return (int)cudaLaunchKernelEx(&cfg, kern, (const uint16_t*)x, perm, (uint16_t*)out, M, K);
+  return launch_kernel(permute_rows_kernel<UNITS>, dim3(M < num_sms() * 8 ? M : num_sms() * 8, 1, 1), dim3(256, 1, 1),
+                       smem, stream, 0, true, (const uint16_t*)x, perm, (uint16_t*)out, M, K);
 }
 
 int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream) {

@@ -35,6 +35,8 @@ def test_abi_argument_validation_without_gpu():
     assert g.lib.b2q_mm_workspace_bytes(1, 4160, 4096, 4, 64, 1) == 4160 * 2   # K % 128 != 0
     assert g.lib.b2q_mm_workspace_bytes(9, 4096, 4096, 4, 128, 1) == 9 * 4096 * 2
     assert g.lib.b2q_mm_workspace_bytes(2, 4096, 4096, 8, 128, 1) == 2 * 4096 * 2
+    assert g.lib.b2q_mm_workspace_bytes(1, 4096, 4096, 8, 32, 1) == 0          # the 8-bit GEMV takes any group size
+    assert g.lib.b2q_mm_workspace_bytes(1, 4160, 4096, 8, 64, 1) == 4160 * 2   # 8-bit, K % 128 != 0: no M=1 tier
     assert g.lib.b2q_mm_workspace_bytes(300, 4096, 4096, 4, 128, 0) == 0
     assert g.lib.b2q_workspace_bytes(16, 4096, 4096, 1) == 16 * 4096 * 2
     assert g.lib.b2q_workspace_bytes(16, 4096, 4096, 0) == 0
@@ -48,6 +50,16 @@ def test_abi_argument_validation_without_gpu():
     assert g.lib.b2q_mm(one, one, one, None, None, None, one, 1, 64, 64, 4, 48, 0, None, 0, None) == -2
     assert b"group_size=48" in g.lib.b2q_last_error()
     assert g.lib.b2q_mm(one, one, one, None, None, None, one, 0, 64, 64, 4, 32, 0, None, 0, None) == 0  # M == 0
+    # b2q_gemv serves exactly the M=1 shapes of the decode tier and the 8-bit GEMV, refused before any CUDA work
+    assert g.lib.b2q_gemv(one, one, one, None, None, None, one, 192, 64, 8, 64, 0, 0, 0, None) == -2  # K % 128 != 0
+    assert b"no M=1 tier" in g.lib.b2q_last_error()
+    assert g.lib.b2q_gemv(one, one, one, None, None, None, one, 128, 64, 4, 32, 0, 0, 0, None) == -2  # 4-bit g32
+    assert b"no M=1 tier" in g.lib.b2q_last_error()
+    for ks, warps in ((3, 0), (32, 0), (0, 17)):  # forced split-K: a power of two <= 16; warps <= 16
+        assert g.lib.b2q_gemv(one, one, one, None, None, None, one, 128, 64, 8, 128, 0, ks, warps, None) == -2
+        assert b"b2q_gemv" in g.lib.b2q_last_error() and b"out of range" in g.lib.b2q_last_error()
+        assert g.lib.b2q_decode(one, one, one, None, None, None, one, 1, 128, 64, 4, 128, 0, ks, warps, None) == -2
+        assert b"b2q_decode" in g.lib.b2q_last_error() and b"out of range" in g.lib.b2q_last_error()
     with pytest.raises(g.B2QError):
         g.check(-2, "x")
 
