@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2q.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 # every symbol include/b2q.h declares: (restype, argtypes)
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
@@ -33,6 +33,7 @@ SYMBOLS = {
     "b2q_decode_allreduce_flag_bytes": (_sz, []),
     "b2q_debug_decode_plan": (_i, [_i, _i, _i, _i, _i, _i, _vp]),
     "b2q_permute_cols": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    "b2q_hadamard": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _vp]),
     "b2q_moe_align": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "b2q_moe_gather": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_moe_gather_perm": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _vp]),

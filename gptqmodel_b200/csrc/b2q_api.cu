@@ -278,6 +278,44 @@ int b2q_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K
   return check_cuda(launch_permute_cols(x, perm, out, M, K, (cudaStream_t)stream), "b2q_permute_cols");
 }
 
+int b2q_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype, void* stream) {
+  if (x == nullptr || out == nullptr || rows < 0) {
+    set_error("b2q_hadamard: bad argument (x, out non-NULL, rows=%d >= 0)", rows);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("b2q_hadamard: dtype=%d not supported (0 fp16, 1 bf16)", dtype);
+    return -2;
+  }
+  if (K < 1 || K > 256 || n <= 0 || n > 65536 || n % K != 0) {
+    set_error("b2q_hadamard: K=%d n=%d outside 1 <= K <= 256, n <= 65536, K dividing n", K, n);
+    return -2;
+  }
+  const int P = n / K;
+  if (P < 8 || (P & (P - 1)) != 0) {
+    set_error("b2q_hadamard: P = n/K = %d must be a power of two >= 8 (n=%d K=%d)", P, n, K);
+    return -2;
+  }
+  if ((had == nullptr) != (K == 1)) {
+    set_error("b2q_hadamard: had must be NULL exactly when K == 1 (K=%d)", K);
+    return -2;
+  }
+  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
+      (reinterpret_cast<uintptr_t>(had) & 15)) {
+    set_error("b2q_hadamard: x, out and had must be 16-byte aligned");
+    return -2;
+  }
+  const uintptr_t xb = reinterpret_cast<uintptr_t>(x), ob = reinterpret_cast<uintptr_t>(out);
+  const uintptr_t bytes = (uintptr_t)rows * (uintptr_t)n * 2;
+  if (xb == ob || (rows > 0 && xb < ob + bytes && ob < xb + bytes)) {
+    set_error("b2q_hadamard: out must not overlap x");
+    return -2;
+  }
+  if (rows == 0) return 0;
+  DeviceGuard dg(out);
+  return check_cuda(launch_hadamard(x, had, K, out, rows, n, dtype, (cudaStream_t)stream), "b2q_hadamard");
+}
+
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
              const void* bias, void* out, int K, int N, int bits, int group_size, int dtype, int ks, int warps,
              void* stream) {

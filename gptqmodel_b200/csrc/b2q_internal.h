@@ -43,6 +43,8 @@ size_t decode_allreduce_flag_bytes();
 
 int launch_prepack(const void* qweight, const int32_t* perm, void* out, int K, int N, int bits, cudaStream_t stream);
 int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream);
+int launch_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype,
+                    cudaStream_t stream);  // b2q_hadamard.cu
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

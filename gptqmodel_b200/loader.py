@@ -45,6 +45,7 @@ class QuantSpec:
     lm_head: bool = False
     dynamic: Optional[Dict[str, dict]] = None
     meta: dict = field(default_factory=dict)
+    rotation: Optional[str] = None  # None | "hadamard" | "random": QuaRot / SpinQuant checkpoint, see load_quantized_linears
 
     def for_module(self, name: str) -> Optional["QuantSpec"]:
         """Per-module view after `dynamic` overrides; None if a negative (`-:`) pattern excludes the module."""
@@ -88,6 +89,7 @@ def parse_quant_config(raw: dict) -> QuantSpec:
     spec.lm_head = bool(d.get("lm_head", False))
     spec.dynamic = d.get("dynamic") or None
     spec.meta = dict(d.get("meta") or {})
+    spec.rotation = d.get("rotation") or None
     pack_dtype = str(d.get("pack_dtype", "int32")).replace("torch.", "")
     if pack_dtype != "int32":
         raise NotImplementedError(f"pack_dtype `{pack_dtype}` is not supported (int32 words only, like Marlin / Swordfish)")
@@ -97,6 +99,12 @@ def parse_quant_config(raw: dict) -> QuantSpec:
         raise NotImplementedError(f"GPTQ checkpoint format `{spec.format}` is not supported (gptq, gptq_v2, gptq_p)")
     if spec.method == "awq" and spec.format != "gemm":
         raise NotImplementedError(f"AWQ checkpoint format `{spec.format}` is not supported (gemm)")
+    # the reference's checks for rotated checkpoints (models/loader.py:283-284, 1392-1396)
+    if spec.rotation is not None:
+        if spec.rotation not in ("hadamard", "random"):
+            raise ValueError(f"Unsupported rotation mode: `{spec.rotation}`")
+        if spec.method != "gptq" or spec.format not in ("gptq", "gptq_v2"):
+            raise NotImplementedError(f"`rotation` is only supported for GPTQ/GPTQ_V2 checkpoints, got `{spec.format}`")
     return spec
 
 
@@ -154,13 +162,56 @@ def _v1_sym_ok(spec: QuantSpec) -> bool:
     return False
 
 
+# Orders of the non-power-of-two Hadamard factor, in the precedence the reference's get_hadK tests them
+# (quantization/rotation/hadamard_utils.py:20-70): the first order dividing n is used, even where a later one would too.
+HADAMARD_ORDERS = (172, 156, 140, 108, 60, 52, 36, 28, 40, 20, 12)
+ROTATED_SUFFIX = "mlp.down_proj"  # the modules that transform their input online (models/loader.py:273-310)
+
+
+def hadamard_order(n: int) -> int:
+    """Order K of the rotation's +-1 factor for a transform of length n = K * 2^m (1: n is a power of two).
+    Raises ValueError for a length the reference cannot rotate either."""
+    def pow2(v):
+        return v > 0 and v & (v - 1) == 0
+
+    for k in HADAMARD_ORDERS:
+        if n % k == 0:
+            if not pow2(n // k):
+                raise ValueError(f"no Hadamard transform of length {n}: {n} / {k} is not a power of two")
+            return k
+    if not pow2(n):
+        raise ValueError(f"no Hadamard transform of length {n}: not a power of two times one of {HADAMARD_ORDERS}")
+    return 1
+
+
+def _hadamard_table(hadamard, order: int, n: int) -> torch.Tensor:
+    """The caller's +-1 matrix of `order` for a transform of length n: `hadamard` maps order -> tensor, or is a callable
+    like the reference's get_hadK(n) -> (tensor, K)."""
+    t = None
+    if callable(hadamard):
+        t, k = hadamard(n)
+        if k != order:
+            t = None
+    elif hadamard is not None:
+        t = hadamard.get(order)
+    if t is None:
+        raise NotImplementedError(f"rotated checkpoint needs the Hadamard matrix of order {order}: pass it in "
+                                  "load_quantized_linears(..., hadamard={order: tensor}) or hadamard=get_hadK")
+    return torch.as_tensor(t)
+
+
 @torch.no_grad()
 def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype] = None,
-                           only: Optional[Iterable[str]] = None, post_init: Optional[bool] = None) -> Dict[str, nn.Module]:
+                           only: Optional[Iterable[str]] = None, post_init: Optional[bool] = None,
+                           hadamard=None) -> Dict[str, nn.Module]:
     """Load every quantised linear of a checkpoint directory into B200 QuantLinear modules.
 
     only      : optional iterable of module prefixes to load (default: all `<prefix>.qweight` found)
     post_init : default True on CUDA devices (prepack for the kernels), False on CPU (tensors only; host tests)
+    hadamard  : rotated checkpoints (`rotation` in the quantisation config) only: the +-1 matrices of the non-power-of-two
+                Hadamard orders, as a mapping {order: tensor [order, order]} or a callable such as the reference's
+                `get_hadK`.  Every `*mlp.down_proj` module gets the reference's online transform of its input; a size whose
+                order has no matrix raises NotImplementedError (power-of-two sizes need none).
     """
     from safetensors import safe_open
 
@@ -214,6 +265,12 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
                                          "(zero-points may have wrapped); the reference refuses it as well")
                     m.qzero_format(1)
                     m.convert_gptq_v1_to_v2()
+                if spec.rotation and prefix.endswith(ROTATED_SUFFIX):
+                    order = hadamard_order(K)
+                    m.online_full_had = True
+                    m.K = order
+                    if order > 1:
+                        m.set_had_K(_hadamard_table(hadamard, order, K))  # validated and copied by post_init()
             if do_post:
                 m.post_init()
             mods[prefix] = m

@@ -122,6 +122,8 @@ def fuse_siblings(mods) -> bool:
             return False
         if m.in_features % 128 != 0 or m._kgs not in (64, 128, m.in_features) or m.adapter:
             return False
+        if m.online_full_had or m.online_partial_had:  # each rotated module transforms its own input
+            return False
     grp = SiblingGroup(mods)
     for m in mods:
         m._siblings = grp
@@ -188,6 +190,14 @@ class B200KernelMixin:
         self._prepacked = False
         self._scales_cache = {}
         self._siblings = None
+        # online Hadamard rotation of the input (QuaRot / SpinQuant checkpoints; the reference's BaseQuantLinear attributes,
+        # qlinear/__init__.py:134-141): the reference-side subclass gets them from its base, which must not be overridden
+        for attr, default in (("online_full_had", False), ("online_partial_had", False), ("had_dim", -1), ("K", 1)):
+            if not hasattr(self, attr):
+                setattr(self, attr, default)
+        if not hasattr(self, "had_K"):
+            self.had_K = None
+        self._had_dev: Optional[torch.Tensor] = None  # had_K as the kernel's int8 [K, K] device array (set_had_K)
 
         K, N, G = in_features, out_features, math.ceil(in_features / self.group_size)
         # checkpoint-shaped, non-trainable Parameters (what Marlin/Swordfish register: swordfish.py:108-148)
@@ -321,6 +331,8 @@ class B200KernelMixin:
         self.g_idx = nn.Parameter(torch.empty(0, dtype=torch.int32, device=dev), requires_grad=False)
         self.scales.data = self.scales.data.contiguous()
         self._prepacked = True
+        if self.had_K is not None:
+            self._had_dev = self._check_had(self.had_K).to(dev)
         base_post_init = getattr(super(), "post_init", None)
         if base_post_init is not None:
             base_post_init()  # reference base: BaseQuantLinear.post_init() initialises the adapter (qlinear/__init__.py:224-234)
@@ -351,6 +363,66 @@ class B200KernelMixin:
             self._scales_cache[key] = c
         return c
 
+    # ---- online Hadamard rotation ------------------------------------------------------------------------
+    def set_had_K(self, had_K: Optional[torch.Tensor]) -> None:
+        """Assign the rotation's +-1 matrix (the reference's `set_had_K`, qlinear/__init__.py:485-504: a non-persistent
+        buffer).  It is validated here; the kernel's device copy is made here after post_init(), else by post_init()."""
+        h8 = None if had_K is None else self._check_had(had_K)
+        if "had_K" in self._buffers:
+            if had_K is None:
+                del self._buffers["had_K"]
+                self.had_K = None
+            else:
+                self._buffers["had_K"] = had_K
+        elif had_K is None:
+            self.had_K = None
+        else:
+            if hasattr(self, "had_K"):
+                del self.had_K
+            self.register_buffer("had_K", had_K, persistent=False)
+        self._had_dev = h8.to(self.packed.device) if h8 is not None and self._prepacked else None
+
+    def _had_length(self) -> int:
+        return self.in_features if self.online_full_had or not self.online_partial_had else self.had_dim
+
+    @torch.no_grad()
+    def _check_had(self, had_K: torch.Tensor) -> torch.Tensor:
+        """Host-side check of had_K (+-1, had_K @ had_K.T == K * I, an order that divides the transformed length into a
+        power of two >= 8); returns it as the int8 [K, K] array b2q_hadamard reads (on the CPU)."""
+        h = torch.as_tensor(had_K).detach().to("cpu", torch.float64)
+        if h.dim() != 2 or h.shape[0] != h.shape[1] or not 1 <= h.shape[0] <= 256:
+            raise ValueError(f"{self.name}: had_K must be a square matrix of order <= 256, got {tuple(h.shape)}")
+        order = h.shape[0]
+        if not bool(((h == 1) | (h == -1)).all()):
+            raise ValueError(f"{self.name}: had_K has entries other than +-1")
+        if not torch.equal(h @ h.T, order * torch.eye(order, dtype=torch.float64)):
+            raise ValueError(f"{self.name}: had_K is not a Hadamard matrix (had_K @ had_K.T != {order} * I)")
+        n = self._had_length()
+        P = n // order if n > 0 and n % order == 0 else 0
+        if P < 8 or P & (P - 1):
+            raise ValueError(f"{self.name}: had_K of order {order} does not fit a transform of length {n} "
+                             "(needs order * a power of two >= 8)")
+        return h.to(torch.int8).contiguous()
+
+    def _rotate(self, x2: torch.Tensor) -> torch.Tensor:
+        """The reference's `_apply_rotation_to_input` (hadamard_utils.py:163-192) on the kernel: rows of `_had_length()`
+        transformed by b2q_hadamard into a new tensor."""
+        K = self.K
+        if self.had_K is None and K != 1:
+            return x2  # the reference leaves x untouched here as well (hadamard_utils.py:176-179)
+        had = None
+        if K != 1:
+            had = self._had_dev
+            if had is None or had.shape[0] != K:
+                raise B2QError(f"{self.name}: had_K of order {K} not prepared; call set_had_K() (or post_init())")
+        n = self._had_length()
+        y = torch.empty_like(x2)
+        if x2.numel() == 0:
+            return y
+        check(lib.b2q_hadamard(x2.data_ptr(), _ptr(had), K, y.data_ptr(), x2.numel() // n, n, _DTYPE_CODE[x2.dtype],
+                               torch.cuda.current_stream(x2.device).cuda_stream), "b2q_hadamard")
+        return y
+
     # ---- hot path ------------------------------------------------------------------------------------
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if not self._prepacked:
@@ -366,6 +438,9 @@ class B200KernelMixin:
         x2 = x.reshape(-1, K)
         if not x2.is_contiguous():
             x2 = x2.contiguous()
+        if self.online_full_had or self.online_partial_had:
+            x2 = self._rotate(x2)
+            x = x2.reshape(x.shape)  # the adapter sees the rotated input, as in the reference (qlinear/torch.py:311-312)
         M = x2.shape[0]
         if self._siblings is not None and (1 <= M <= DECODE_MAX_M or M > PREFILL_MIN_M):
             return self._siblings.run(self, x2, M).reshape(out_shape)
@@ -409,6 +484,8 @@ class B200KernelMixin:
         if not (1 <= M <= DECODE_MAX_M) or self.kbits != 4 or self.perm is not None or self._gather is not None \
                 or x.dtype not in _DTYPE_CODE:
             raise B2QError("forward_allreduce: decode tier only (bits=4, 1 <= tokens <= 8, no act-order, fp16/bf16)")
+        if self.online_full_had or self.online_partial_had:
+            raise B2QError("forward_allreduce: a row shard cannot apply an online Hadamard transform over all input columns")
         if self.adapter:
             # the adapter's low-rank update belongs to the FULL layer output; applying it to one rank's partial sum (or
             # dropping it silently, ADVICE r01) would change the result: callers use forward() + all-reduce instead

@@ -241,6 +241,9 @@ class RowParallelLinear(torch.nn.Module):
 
     def __init__(self, inner: torch.nn.Module, group: Optional[dist.ProcessGroup] = None, reduce=None,
                  overlap_chunks: int = 1, overlap_min_tokens: int = 1024):
+        if getattr(inner, "online_full_had", False) or getattr(inner, "online_partial_had", False):
+            # the online Hadamard transform mixes all K input columns; a row shard holds K / world of them
+            raise NotImplementedError("RowParallelLinear: rotated layers (online Hadamard transform) cannot be row-sharded")
         super().__init__()
         self.inner = inner
         self.group = group

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 5
+#define B2Q_ABI_VERSION 6
 #define B2Q_DTYPE_F16 0
 #define B2Q_DTYPE_BF16 1
 
@@ -196,6 +196,16 @@ int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, i
 
 /* out[m, k'] = x[m, perm[k']] for 16-bit elements. */
 int b2q_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, void* stream);
+
+/* Online Hadamard transform of a rotated (QuaRot / SpinQuant) layer's input (ABI v6): for each of `rows` rows v of
+ * length n = K * P, P a power of two,
+ *   out = vec(had . V . H_P) / sqrt(n),   V = v viewed as [K, P] row-major,  H_P[i, j] = (-1)^popcount(i & j)
+ * the reference's matmul_hadU (gptqmodel/quantization/rotation/hadamard_utils.py), computed in fp32 and rounded once.
+ *   had   : int8 +-1 [K, K] row-major, 16-byte aligned; NULL exactly when K == 1
+ *   x, out: fp16 (dtype 0) or bf16 (dtype 1) [rows, n], 16-byte aligned, out must not overlap x
+ * Requires 1 <= K <= 256, P >= 8, n <= 65536, rows >= 0 (0: no-op).  Deterministic.  Launched with programmatic dependent
+ * launch, so a following b2q_mm / b2q_decode may start loading its weights while the transform runs. */
+int b2q_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype, void* stream);
 
 #ifdef __cplusplus
 }
