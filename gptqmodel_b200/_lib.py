@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2q.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 # every symbol include/b2q.h declares: (restype, argtypes)
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
@@ -43,6 +43,12 @@ SYMBOLS = {
     "b2q_moe_decode_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "b2q_moe_decode_act": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "b2q_moe_decode_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b2q_qqq_packed_bytes": (_sz, [_i, _i]),
+    "b2q_qqq_workspace_bytes": (_sz, [_i, _i]),
+    "b2q_qqq_prepack": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "b2q_qqq_quantize": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b2q_qqq_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b2q_qqq_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
 }
 
 

@@ -316,6 +316,136 @@ int b2q_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, i
   return check_cuda(launch_hadamard(x, had, K, out, rows, n, dtype, (cudaStream_t)stream), "b2q_hadamard");
 }
 
+// ---- QQQ (W4A8) tier ----
+static size_t qqq_kp(int K) { return ((size_t)K + 127) / 128 * 128; }
+static size_t qqq_scale_bytes(int M) { return ((size_t)M * 4 + 127) / 128 * 128; }
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// the reference's IN_OUTPUT_FEATURES_DIVISIBLE_BY, K <= 65536 (exact int32 sums), group size -1 or 128
+static int qqq_check_shape(const char* fn, int M, int K, int N, int group_size) {
+  const bool env_ok = (K % 128 == 0 && N % 64 == 0) || (K % 64 == 0 && N % 128 == 0);
+  if (M < 0 || K <= 0 || N <= 0 || K > 65536 || !env_ok) {
+    set_error("%s: shape M=%d K=%d N=%d outside the envelope (K %% 128 == 0 and N %% 64 == 0, or K %% 64 == 0 and "
+              "N %% 128 == 0; K <= 65536)", fn, M, K, N);
+    return -2;
+  }
+  if (group_size != -1 && !(group_size == 128 && K % 128 == 0)) {
+    set_error("%s: group_size=%d not supported for K=%d (-1, or 128 dividing K)", fn, group_size, K);
+    return -2;
+  }
+  return 0;
+}
+
+size_t b2q_qqq_packed_bytes(int K, int N) {
+  if (K <= 0 || N <= 0) return 0;
+  return qqq_kp(K) * (((size_t)N + 127) / 128 * 128) / 2;
+}
+
+size_t b2q_qqq_workspace_bytes(int M, int K) {
+  if (M <= 0 || K <= 0) return 0;
+  return qqq_scale_bytes(M) + (size_t)M * qqq_kp(K);
+}
+
+int b2q_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int group_size, void* stream) {
+  if (codes == nullptr || packed == nullptr) {
+    set_error("b2q_qqq_prepack: null pointer argument");
+    return -2;
+  }
+  if (int e = qqq_check_shape("b2q_qqq_prepack", 0, K, N, group_size)) return e;
+  if (!aligned16(packed)) {
+    set_error("b2q_qqq_prepack: packed must be 16-byte aligned");
+    return -2;
+  }
+  DeviceGuard dg(packed);
+  return check_cuda(launch_qqq_prepack(codes, packed, K, N, group_size == 128 ? 1 : 0, (cudaStream_t)stream),
+                    "b2q_qqq_prepack");
+}
+
+int b2q_qqq_quantize(const void* x, int8_t* q, float* s_tok, int M, int K, int dtype, void* stream) {
+  if ((M > 0 && (x == nullptr || q == nullptr || s_tok == nullptr)) || M < 0 || K <= 0 || K % 64 != 0 || K > 65536) {
+    set_error("b2q_qqq_quantize: bad argument (non-NULL pointers, M=%d >= 0, K=%d a multiple of 64 <= 65536)", M, K);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("b2q_qqq_quantize: dtype=%d not supported (0 fp16, 1 bf16)", dtype);
+    return -2;
+  }
+  if (!aligned16(x) || !aligned16(q)) {
+    set_error("b2q_qqq_quantize: x and q must be 16-byte aligned");
+    return -2;
+  }
+  if (M == 0) return 0;
+  DeviceGuard dg(q);
+  return check_cuda(launch_qqq_quant(x, q, s_tok, M, K, dtype, (cudaStream_t)stream), "b2q_qqq_quantize");
+}
+
+static int qqq_mm(const char* fn, const int8_t* q, const float* s_tok, const void* packed, const float* s_channel,
+                  const void* s_group, const void* bias, void* out, int M, int K, int N, int out_dtype,
+                  cudaStream_t stream) {
+  QqqArgs a = {q, s_tok, packed, s_channel, s_group, bias, out, M, K, N, out_dtype, stream};
+  return check_cuda(launch_qqq_gemm(a), fn);
+}
+
+static int qqq_check_mm(const char* fn, const void* packed, const float* s_channel, const void* s_group, void* out,
+                        int M, int K, int N, int group_size, int out_dtype) {
+  if (packed == nullptr || s_channel == nullptr || out == nullptr) {
+    set_error("%s: null pointer argument", fn);
+    return -2;
+  }
+  if (int e = qqq_check_shape(fn, M, K, N, group_size)) return e;
+  if ((group_size == 128) != (s_group != nullptr)) {
+    set_error("%s: s_group must be given exactly for group_size 128 (group_size=%d)", fn, group_size);
+    return -2;
+  }
+  if (out_dtype != B2Q_DTYPE_F16 && out_dtype != B2Q_DTYPE_BF16) {
+    set_error("%s: dtype=%d not supported (0 fp16, 1 bf16)", fn, out_dtype);
+    return -2;
+  }
+  if (!aligned16(packed) || !aligned16(out) || !aligned16(s_channel)) {
+    set_error("%s: packed, out and s_channel must be 16-byte aligned", fn);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_qqq_mm(const int8_t* q, const float* s_tok, const void* packed, const float* s_channel, const void* s_group,
+               const void* bias, void* out, int M, int K, int N, int group_size, int out_dtype, void* stream) {
+  if (int e = qqq_check_mm("b2q_qqq_mm", packed, s_channel, s_group, out, M, K, N, group_size, out_dtype)) return e;
+  if (M > 0 && (q == nullptr || s_tok == nullptr || !aligned16(q))) {
+    set_error("b2q_qqq_mm: q (16-byte aligned) and s_tok must be given");
+    return -2;
+  }
+  if (M == 0) return 0;
+  DeviceGuard dg(packed);
+  return qqq_mm("b2q_qqq_mm", q, s_tok, packed, s_channel, s_group, bias, out, M, K, N, out_dtype,
+                (cudaStream_t)stream);
+}
+
+int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, const void* s_group, const void* bias,
+                    void* out, int M, int K, int N, int group_size, int dtype, int out_dtype, void* workspace,
+                    size_t workspace_bytes, void* stream) {
+  if (int e = qqq_check_mm("b2q_qqq_forward", packed, s_channel, s_group, out, M, K, N, group_size, out_dtype))
+    return e;
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("b2q_qqq_forward: dtype=%d not supported (0 fp16, 1 bf16)", dtype);
+    return -2;
+  }
+  if (M == 0) return 0;
+  if (x == nullptr || !aligned16(x) || workspace == nullptr || !aligned16(workspace) ||
+      workspace_bytes < b2q_qqq_workspace_bytes(M, K)) {
+    set_error("b2q_qqq_forward: x and a workspace of b2q_qqq_workspace_bytes(M, K) = %zu bytes (16-byte aligned) "
+              "must be given, got %zu", b2q_qqq_workspace_bytes(M, K), workspace_bytes);
+    return -2;
+  }
+  DeviceGuard dg(packed);
+  float* s_tok = reinterpret_cast<float*>(workspace);
+  int8_t* q = reinterpret_cast<int8_t*>(workspace) + qqq_scale_bytes(M);
+  int e = check_cuda(launch_qqq_quant(x, q, s_tok, M, K, dtype, (cudaStream_t)stream), "b2q_qqq_forward");
+  if (e != 0) return e;
+  return qqq_mm("b2q_qqq_forward", q, s_tok, packed, s_channel, s_group, bias, out, M, K, N, out_dtype,
+                (cudaStream_t)stream);
+}
+
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
              const void* bias, void* out, int K, int N, int bits, int group_size, int dtype, int ks, int warps,
              void* stream) {

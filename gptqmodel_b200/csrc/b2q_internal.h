@@ -45,6 +45,21 @@ int launch_prepack(const void* qweight, const int32_t* perm, void* out, int K, i
 int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream);
 int launch_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype,
                     cudaStream_t stream);  // b2q_hadamard.cu
+// QQQ (W4A8) tier (b2q_qqq.cu)
+struct QqqArgs {
+  const void* q;          // int8 codes [M, Kp], Kp = K rounded up to 128
+  const float* s_tok;     // [M]
+  const void* packed;     // b2q_qqq_prepack tiles
+  const float* s_channel; // [N]
+  const void* s_group;    // fp16 [K/128, N] or nullptr (per-channel)
+  const void* bias;       // fp16 [N] or nullptr
+  void* out;              // [M, N], fp16 (out_dtype 0) or bf16 (1)
+  int M, K, N, out_dtype;
+  cudaStream_t stream;
+};
+int launch_qqq_quant(const void* x, void* q, float* s_tok, int M, int K, int dtype, cudaStream_t stream);
+int launch_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int grouped, cudaStream_t stream);
+int launch_qqq_gemm(const QqqArgs& a);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

@@ -8,7 +8,8 @@ What the reference does for this step, restated for this package (no model defin
   * ``dynamic`` maps module-name regexes to per-module overrides; the FIRST matching pattern wins, a ``-:`` prefix means
     "this module is not quantised", ``+:`` is an explicit positive match (config.py:1579-1652, 1822-1854);
   * a quantised linear ``<prefix>`` is stored as ``<prefix>.qweight / .qzeros / .scales / .g_idx [/ .bias]``
-    (nn_modules/qlinear/__init__.py:827-865); AWQ GEMM checkpoints have no ``g_idx`` (:1634-1668);
+    (nn_modules/qlinear/__init__.py:827-865); AWQ GEMM checkpoints have no ``g_idx`` (:1634-1668); QQQ (W4A8)
+    checkpoints store ``<prefix>.B / .s_channel / .s_group [/ .bias]`` (nn_modules/qlinear/qqq.py);
   * ``format == "gptq"`` files hold v1 zero-points (stored as zero - 1): kernels that need the true zero-point get
     ``qzeros += 0x11111111`` (4-bit) / ``0x01010101`` (8-bit) at load (utils/model.py:800-846, models/loader.py:1657-1675);
     the reference refuses asymmetric v1 files that were not produced by its own >= 0.9.0 quantiser (loader.py:1659-1663).
@@ -41,7 +42,7 @@ class QuantSpec:
     desc_act: bool = False
     sym: bool = True
     format: str = "gptq"   # "gptq" (v1 zero-points) | "gptq_v2" | "gptq_p" (planar, v2 zero-points) | "gemm" (AWQ)
-    method: str = "gptq"   # "gptq" | "awq"
+    method: str = "gptq"   # "gptq" | "awq" | "qqq"
     lm_head: bool = False
     dynamic: Optional[Dict[str, dict]] = None
     meta: dict = field(default_factory=dict)
@@ -93,8 +94,12 @@ def parse_quant_config(raw: dict) -> QuantSpec:
     pack_dtype = str(d.get("pack_dtype", "int32")).replace("torch.", "")
     if pack_dtype != "int32":
         raise NotImplementedError(f"pack_dtype `{pack_dtype}` is not supported (int32 words only, like Marlin / Swordfish)")
-    if spec.method not in ("gptq", "awq"):
-        raise NotImplementedError(f"quantisation method `{spec.method}` is outside this package (gptq, awq)")
+    if spec.method not in ("gptq", "awq", "qqq"):
+        raise NotImplementedError(f"quantisation method `{spec.method}` is outside this package (gptq, awq, qqq)")
+    if spec.method == "qqq":
+        if fmt is None:
+            spec.format = "qqq"
+        _check_qqq(spec)
     if spec.method == "gptq" and spec.format not in ("gptq", "gptq_v2", "gptq_p"):
         raise NotImplementedError(f"GPTQ checkpoint format `{spec.format}` is not supported (gptq, gptq_v2, gptq_p)")
     if spec.method == "awq" and spec.format != "gemm":
@@ -106,6 +111,17 @@ def parse_quant_config(raw: dict) -> QuantSpec:
         if spec.method != "gptq" or spec.format not in ("gptq", "gptq_v2"):
             raise NotImplementedError(f"`rotation` is only supported for GPTQ/GPTQ_V2 checkpoints, got `{spec.format}`")
     return spec
+
+
+def _check_qqq(spec: QuantSpec) -> None:
+    """QQQ (W4A8) checkpoints: 4-bit, symmetric, group size -1 or 128 (the reference's QQQLinear), no rotation."""
+    if spec.format != "qqq":
+        raise NotImplementedError(f"QQQ checkpoint format `{spec.format}` is not supported (qqq)")
+    if spec.bits != 4 or spec.group_size not in (-1, 128) or not spec.sym:
+        raise NotImplementedError(f"QQQ: bits={spec.bits} group_size={spec.group_size} sym={spec.sym} unsupported "
+                                  "(4-bit, group size -1 or 128, symmetric)")
+    if spec.rotation is not None:
+        raise NotImplementedError("`rotation` is not supported for QQQ checkpoints")
 
 
 def read_quant_config(path: str) -> QuantSpec:
@@ -145,6 +161,12 @@ def _weight_map(path: str) -> Dict[str, str]:
 def quantized_prefixes(names: Iterable[str]) -> list:
     """Module prefixes that carry a packed weight (`<prefix>.qweight`)."""
     return sorted(n[: -len(".qweight")] for n in names if n.endswith(".qweight"))
+
+
+def qqq_prefixes(names: Iterable[str]) -> list:
+    """Module prefixes of a QQQ checkpoint (`<prefix>.B` together with `<prefix>.s_channel`)."""
+    names = set(names)
+    return sorted(n[: -len(".s_channel")] for n in names if n.endswith(".s_channel") and n[: -len(".s_channel")] + ".B" in names)
 
 
 def _v1_sym_ok(spec: QuantSpec) -> bool:
@@ -217,10 +239,14 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
 
     from .awq import B200AwqQuantLinear
     from .qlinear import B200QuantLinear
+    from .qqq import B200QqqQuantLinear
 
     spec = read_quant_config(path)
     wmap = _weight_map(path)
-    prefixes = quantized_prefixes(wmap) if only is None else list(only)
+    if only is not None:
+        prefixes = list(only)
+    else:
+        prefixes = qqq_prefixes(wmap) if spec.method == "qqq" else quantized_prefixes(wmap)
     dev = torch.device(device)
     do_post = (dev.type == "cuda") if post_init is None else post_init
     handles: Dict[str, object] = {}
@@ -239,6 +265,22 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
             ms = spec.for_module(prefix)
             if ms is None:
                 continue  # excluded by a negative dynamic pattern: stays a dense layer in the model
+            if ms.method == "qqq":
+                _check_qqq(ms)  # a `dynamic` override may have changed bits / group size
+                t = {s: tensor(f"{prefix}.{s}") for s in ("B", "s_channel", "s_group", "bias")}
+                if t["B"] is None or t["s_channel"] is None:
+                    raise KeyError(f"{prefix}: checkpoint misses B / s_channel")
+                K, N = t["B"].shape[0] * 16, t["B"].shape[1] // 2
+                m = B200QqqQuantLinear(bits=4, group_size=ms.group_size, desc_act=ms.desc_act, sym=True, in_features=K,
+                                       out_features=N, bias=t["bias"] is not None, register_buffers=False, dtype=dtype,
+                                       name=prefix)
+                sg = t["s_group"] if t["s_group"] is not None else torch.empty(0, dtype=torch.float16)
+                m.B, m.s_channel, m.s_group = t["B"].to(dev), t["s_channel"].to(dev, torch.float32), sg.to(dev)
+                m.bias = None if t["bias"] is None else t["bias"].to(dev, torch.float16)
+                if do_post:
+                    m.post_init()
+                mods[prefix] = m
+                continue
             t = {s: tensor(f"{prefix}.{s}") for s in _TENSOR_SUFFIXES}
             if t["qweight"] is None or t["qzeros"] is None or t["scales"] is None:
                 raise KeyError(f"{prefix}: checkpoint misses qweight / qzeros / scales")

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 6
+#define B2Q_ABI_VERSION 7
 #define B2Q_DTYPE_F16 0
 #define B2Q_DTYPE_BF16 1
 
@@ -206,6 +206,33 @@ int b2q_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K
  * Requires 1 <= K <= 256, P >= 8, n <= 65536, rows >= 0 (0: no-op).  Deterministic.  Launched with programmatic dependent
  * launch, so a following b2q_mm / b2q_decode may start loading its weights while the transform runs. */
 int b2q_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype, void* stream);
+
+/* QQQ (W4A8) tier (ABI v7): 4-bit weights, per-token int8 activations, int8 tensor cores (b2q_qqq.cu).  The arithmetic
+ * of the reference's QQQLinear.forward + qqq_gemm (gptqmodel/nn_modules/qlinear/qqq.py, gptqmodel_ext/qqq):
+ *   A = fp16(x);  s_tok[m] = fp32(fp16(max_k |A[m,k]| / 127));  q[m,k] = clamp(rint(A[m,k] / s_tok[m]), -128, 127)
+ *   (IEEE fp32 division; an all-zero row gets s_tok = 0 and codes 0);
+ *   w[k,n] = signed code * 16 (group_size -1) or round_half_even((code - 8) * s_group[k/128, n]) (group_size 128);
+ *   acc = sum_k q * w in int32 (exact);  y = fp16(fp32(acc) * s_channel[n] * s_tok[m]);  y = fp16(y + bias[n]);
+ *   bf16 output (out_dtype 1) = bf16(y).
+ * Shapes: K % 128 == 0 and N % 64 == 0, or K % 64 == 0 and N % 128 == 0; K <= 65536; group_size -1, or 128 dividing K.
+ * Tensors: codes uint8 [K, N] (canonical 4-bit codes, one per byte), s_channel fp32 [N] (16-byte aligned),
+ * s_group fp16 [K/128, N] (NULL exactly for group_size -1), bias fp16 [N] or NULL.  Deterministic for any launch split. */
+size_t b2q_qqq_packed_bytes(int K, int N);
+/* Workspace of b2q_qqq_forward: the token scales and int8 codes of M rows. */
+size_t b2q_qqq_workspace_bytes(int M, int K);
+/* One-time repack of canonical codes into the kernel's tile layout (zero-padded to 128 k and 128 features). */
+int b2q_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int group_size, void* stream);
+/* Activation quantiser: x fp16/bf16 [M, K] -> q int8 [M, K rounded up to 128] (padding codes 0), s_tok fp32 [M].
+ * Launched with programmatic dependent launch, so a following b2q_qqq_mm starts streaming its weights meanwhile. */
+int b2q_qqq_quantize(const void* x, int8_t* q, float* s_tok, int M, int K, int dtype, void* stream);
+/* out[M, N] from codes and token scales (b2q_qqq_quantize's output). */
+int b2q_qqq_mm(const int8_t* q, const float* s_tok, const void* packed, const float* s_channel, const void* s_group,
+               const void* bias, void* out, int M, int K, int N, int group_size, int out_dtype, void* stream);
+/* b2q_qqq_quantize + b2q_qqq_mm through a caller workspace of b2q_qqq_workspace_bytes(M, K) bytes (16-byte aligned);
+ * dispatches on M inside the library, so a CUDA graph sees the true M. */
+int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, const void* s_group, const void* bias,
+                    void* out, int M, int K, int N, int group_size, int dtype, int out_dtype, void* workspace,
+                    size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
