@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2q.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 # every symbol include/b2q.h declares: (restype, argtypes)
 _vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
@@ -49,6 +49,8 @@ SYMBOLS = {
     "b2q_qqq_quantize": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_qqq_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b2q_qqq_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "b2q_fp8_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "b2q_fp8_dequant": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
 }
 
 

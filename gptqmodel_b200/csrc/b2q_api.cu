@@ -129,6 +129,7 @@ static MmArgs make_args(const void* x, const void* packed, const void* scales, c
   a.stream = (cudaStream_t)stream;
   a.tune_ks = 0;
   a.tune_warps = 0;
+  a.fp8 = 0;
   return a;
 }
 
@@ -444,6 +445,56 @@ int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, c
   if (e != 0) return e;
   return qqq_mm("b2q_qqq_forward", q, s_tok, packed, s_channel, s_group, bias, out, M, K, N, out_dtype,
                 (cudaStream_t)stream);
+}
+
+// ---- FP8 (e4m3fn, W8A16) layers on the 8-bit tiers ----
+static int fp8_check(const char* fn, const void* packed, const void* scales, const void* out, int K, int N,
+                     int group_size, int dtype) {
+  if (packed == nullptr || scales == nullptr || out == nullptr) {
+    set_error("%s: null pointer argument", fn);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("%s: dtype=%d not supported (0 fp16, 1 bf16)", fn, dtype);
+    return -2;
+  }
+  if (K <= 0 || N <= 0 || K % 64 != 0 || N % 32 != 0) {
+    set_error("%s: shape K=%d N=%d not supported (K multiple of 64, N multiple of 32)", fn, K, N);
+    return -2;
+  }
+  if (!((group_size == 64 || group_size == 128 || group_size == K) && K % group_size == 0)) {
+    set_error("%s: group_size=%d not supported for K=%d (64 | 128 dividing K, or K)", fn, group_size, K);
+    return -2;
+  }
+  if (!aligned16(packed) || !aligned16(out)) {
+    set_error("%s: packed and out must be 16-byte aligned", fn);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_fp8_mm(const void* x, const void* packed, const void* scales, const void* bias, void* out, int M, int K, int N,
+               int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int e = fp8_check("b2q_fp8_mm", packed, scales, out, K, N, group_size, dtype)) return e;
+  if (M < 0 || (M > 0 && (x == nullptr || !aligned16(x)))) {
+    set_error("b2q_fp8_mm: M=%d must be >= 0 and x a 16-byte aligned pointer", M);
+    return -2;
+  }
+  if (M == 0) return 0;
+  DeviceGuard dg(packed);
+  MmArgs a = make_args(x, packed, scales, nullptr, nullptr, bias, out, M, K, N, 8, group_size, dtype, workspace,
+                       workspace_bytes, stream);
+  a.fp8 = 1;
+  if (gemv_supported(a)) return check_cuda(launch_gemv(a), "b2q_fp8_mm(gemv)");
+  return check_cuda(launch_gemm(a), "b2q_fp8_mm(gemm)");
+}
+
+int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
+                    void* stream) {
+  if (int e = fp8_check("b2q_fp8_dequant", packed, scales, out, K, N, group_size, dtype)) return e;
+  DeviceGuard dg(packed);
+  return check_cuda(launch_fp8_dequant(packed, scales, out, K, N, group_size, dtype, (cudaStream_t)stream),
+                    "b2q_fp8_dequant");
 }
 
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,

@@ -1,5 +1,8 @@
-// b2q_dequant.cuh — exact (q - z) * s dequantisation of packed B2Q words for the tensor-core tiers.
+// b2q_dequant.cuh — exact (q - z) * s dequantisation of packed B2Q words for the tensor-core tiers, and the exact
+// e4m3 / scale division of FP8 layers.
 #pragma once
+#include <cuda_fp8.h>
+
 #include "b2q_common.cuh"
 
 namespace b2q {
@@ -133,5 +136,69 @@ struct Dequant<__nv_bfloat16, 8> {
   }
 };
 
+// ---- FP8 (e4m3fn) weights: W = T(w) / T(scale_inv), one correctly rounded division per weight ------------------------
+// Two e4m3 codes (low byte first) -> the exact half2 of their values: every e4m3fn value, NaN included, is an fp16 value.
+__device__ __forceinline__ __half2 e4m3x2_to_h2(uint32_t two_bytes) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(two_bytes & 0xFFFFu), __NV_E4M3);
+  return *reinterpret_cast<const __half2*>(&h);
+}
+
+// Divisor of one quantisation group: s = float(T scale), r = RN32(1 / s).  For |s| in [2^-100, 2^100] (every fp16 value,
+// and every bf16 scale a real checkpoint carries) q0 = w r, e = w - q0 s (exact), q = q0 + e r is RN32(w / s) for every
+// e4m3 w (Markstein: r correctly rounded, q0 faithful).  RN_T of it is RN_T(w / s): an fp32 quotient rounded to a 16-bit
+// type is not a double rounding (24 >= 2 * 11 + 2), and it is what torch computes for T(w) / T(s).  Outside that range
+// (bf16 scales, and an fp16 scale that overflowed to inf) the reciprocal over- or underflows and the IEEE division is
+// used instead.
+struct Fp8Div {
+  float s, r;
+  bool fast;
+};
+
+template <typename T>
+__device__ __forceinline__ Fp8Div fp8_div_of(uint32_t s16) {
+  Fp8Div d;
+  d.s = ET<T>::to_f(*reinterpret_cast<const T*>(&s16));
+  d.r = __frcp_rn(d.s);
+  const uint32_t ex = (__float_as_uint(d.s) >> 23) & 0xFFu;
+  d.fast = ex >= 127u - 100u && ex <= 127u + 100u;
+  return d;
+}
+
+// The remainder is formed negated (q0 s - w) so that a zero weight keeps its sign: -0 / s = -0, as torch computes it.
+__device__ __forceinline__ float fp8_div_fast(float w, const Fp8Div& d) {
+  const float q0 = __fmul_rn(w, d.r);
+  const float en = fmaf(q0, d.s, -w);
+  return fmaf(-en, d.r, q0);
+}
+
+// 16 consecutive k of one feature (one T8 uint4, natural byte order) -> 2 x uint4 of T, the same layout Dequant<T, 8>
+// produces.
+template <typename T>
+struct DequantFp8 {
+  __device__ static __forceinline__ void run(const uint4& pv, const Fp8Div& d, uint4 (&o)[2]) {
+    const uint32_t w[4] = {pv.x, pv.y, pv.z, pv.w};
+    float f[16];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float2 a = __half22float2(e4m3x2_to_h2(w[t])), b = __half22float2(e4m3x2_to_h2(w[t] >> 16));
+      f[4 * t] = a.x;
+      f[4 * t + 1] = a.y;
+      f[4 * t + 2] = b.x;
+      f[4 * t + 3] = b.y;
+    }
+    if (d.fast) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) f[i] = fp8_div_fast(f[i], d);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) f[i] = __fdiv_rn(f[i], d.s);
+    }
+    uint32_t r[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r[i] = ET<T>::pack2(f[2 * i], f[2 * i + 1]);
+    o[0] = make_uint4(r[0], r[1], r[2], r[3]);
+    o[1] = make_uint4(r[4], r[5], r[6], r[7]);
+  }
+};
 
 }  // namespace b2q

@@ -23,7 +23,7 @@
 
 namespace b2q {
 
-template <typename T, int BITS, bool ASYM, int STAGES>
+template <typename T, int BITS, bool ASYM, int STAGES, bool FP8 = false>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ GemmSets S, int M, int K,
                 int gshc) {
@@ -231,13 +231,18 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         for (int j = 0; j < 2; ++j) {
           int z = ZSYM;
           if (ASYM) z = (int)((cur[j].zw >> (BITS * (nsafe % PF))) & ((1u << BITS) - 1));
+          Fp8Div dv = {};
+          if constexpr (FP8) dv = fp8_div_of<T>(cur[j].s);
           const uint4* pj = reinterpret_cast<const uint4*>(smem + (sP - smem_base) + s * C::P_BYTES +
                                                            j * C::P_CHUNK_BYTES);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const uint4 pv = pj[(ntl * 2 + h) * 32 + lane];
             uint4 o[2];
-            Dequant<T, 8>::run(pv, cur[j].s, z, o);
+            if constexpr (FP8)
+              DequantFp8<T>::run(pv, dv, o);
+            else
+              Dequant<T, 8>::run(pv, cur[j].s, z, o);
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
               const uint32_t addr = brow + (((uint32_t)(j * 4 + h * 2 + c) ^ sw) << 4);
@@ -336,12 +341,12 @@ int gemm_gshc(const MmArgs& a) {
 }
 
 
-template <typename T, int BITS, bool ASYM, int STAGES>
+template <typename T, int BITS, bool ASYM, int STAGES, bool FP8 = false>
 static int launch_gemm_t(const MmArgs& a, const void* x, const GemmSets& S) {
   using C = GemmCfg<BITS, STAGES>;
   CUtensorMap tmap;
   if (make_x_tmap(&tmap, x, a.M, a.K, a.dtype) != 0) return -1;
-  auto kern = gemm_kernel<T, BITS, ASYM, STAGES>;
+  auto kern = gemm_kernel<T, BITS, ASYM, STAGES, FP8>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_gemm")) return e;
   dim3 grid(S.tn_end[S.nsets - 1], (a.M + G_BM - 1) / G_BM, 1);
@@ -350,6 +355,9 @@ static int launch_gemm_t(const MmArgs& a, const void* x, const GemmSets& S) {
 }
 
 static int launch_gemm_sets(const MmArgs& a, const void* x, const GemmSets& S) {
+  // FP8 layers: 8-bit codes, no zero-points, the e4m3 / scale division in the dequant warpgroup
+  if (a.fp8) return a.dtype == 0 ? launch_gemm_t<__half, 8, false, 4, true>(a, x, S)
+                                 : launch_gemm_t<__nv_bfloat16, 8, false, 4, true>(a, x, S);
   const bool asym = S.qzeros[0] != nullptr;
 #define B2Q_GEMM_CASE(T, BITS, ST) \
   (asym ? launch_gemm_t<T, BITS, true, ST>(a, x, S) : launch_gemm_t<T, BITS, false, ST>(a, x, S))

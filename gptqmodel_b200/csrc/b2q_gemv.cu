@@ -12,6 +12,7 @@
 //  * act-order: rows sorted by group at prepack; the x[perm[k']] gather is fused into the smem staging.
 // Replaces, for 8-bit M == 1, TorchLinear.forward (qlinear/torch.py:302-347) / Marlin's small-M path.
 #include "b2q_common.cuh"
+#include "b2q_dequant.cuh"
 #include "b2q_internal.h"
 
 namespace b2q {
@@ -60,7 +61,7 @@ __device__ __forceinline__ void load_quad(Quad<T, BITS, ASYM>& q, const uint4* _
 
 // dot of one 32-k chunk of one feature with the staged activations; returns sum (BASE+q)*x split in the two
 // magic-number classes (lo: BASE = LO_BASE, hi: BASE = HI_BASE after HI_SCALE).
-template <typename T, int BITS>
+template <typename T, int BITS, bool FP8 = false>
 __device__ __forceinline__ void chunk_dot(const uint4* v, const uint4* __restrict__ xs, float& lo, float& hi) {
   using E = ET<T>;
   float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
@@ -74,7 +75,21 @@ __device__ __forceinline__ void chunk_dot(const uint4* v, const uint4* __restric
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
         const uint2 xv = reinterpret_cast<const uint2*>(xs)[hsub * 4 + t];  // x[16h+4t .. +3]
-        if (E::FMT == 0) {
+        if (FP8) {
+          // e4m3 codes: the exact half pair of (k0,k1) / (k2,k3), no bias; x widened exactly
+          const __half2 p0 = e4m3x2_to_h2(w[t]), p1 = e4m3x2_to_h2(w[t] >> 16);
+          if (E::FMT == 0) {
+            a0 = E::fma_lo(*reinterpret_cast<const uint32_t*>(&p0), xv.x, a0);
+            a1 = E::fma_hi(*reinterpret_cast<const uint32_t*>(&p0), xv.x, a1);
+            b0 = E::fma_lo(*reinterpret_cast<const uint32_t*>(&p1), xv.y, b0);
+            b1 = E::fma_hi(*reinterpret_cast<const uint32_t*>(&p1), xv.y, b1);
+          } else {
+            a0 = fmaf(__low2float(p0), __uint_as_float(xv.x << 16), a0);
+            a1 = fmaf(__high2float(p0), __uint_as_float(xv.x & 0xFFFF0000u), a1);
+            b0 = fmaf(__low2float(p1), __uint_as_float(xv.y << 16), b0);
+            b1 = fmaf(__high2float(p1), __uint_as_float(xv.y & 0xFFFF0000u), b1);
+          }
+        } else if (E::FMT == 0) {
           const uint32_t p0 = __byte_perm(w[t], 0x64006400u, 0x7150);
           const uint32_t p1 = __byte_perm(w[t], 0x64006400u, 0x7352);
           a0 = E::fma_lo(p0, xv.x, a0);
@@ -96,7 +111,7 @@ __device__ __forceinline__ void chunk_dot(const uint4* v, const uint4* __restric
   }
 }
 
-template <typename T, int BITS, bool ASYM, bool PERM>
+template <typename T, int BITS, bool ASYM, bool PERM, bool FP8 = false>
 __global__ void __launch_bounds__(GEMV_MAX_WARPS * 32)
     gemv_kernel(const uint4* __restrict__ packed, const T* __restrict__ scales, const uint32_t* __restrict__ qzeros,
                 const int32_t* __restrict__ perm, const T* __restrict__ x, const T* __restrict__ bias,
@@ -184,7 +199,7 @@ __global__ void __launch_bounds__(GEMV_MAX_WARPS * 32)
     for (int j = 0; j < 4; ++j) {
       const int kc = q + j;
       if (kc < c1) {
-        chunk_dot<T, BITS>(&cur.v[j * (BITS / 4)], reinterpret_cast<const uint4*>(sx + (kc - c0) * 32), lo, hi);
+        chunk_dot<T, BITS, FP8>(&cur.v[j * (BITS / 4)], reinterpret_cast<const uint4*>(sx + (kc - c0) * 32), lo, hi);
         const float2 cs = csum[kc - c0];
         cl += cs.x;
         ch += cs.y;
@@ -192,6 +207,12 @@ __global__ void __launch_bounds__(GEMV_MAX_WARPS * 32)
         if (group_end) {
           const uint16_t sraw = cur.s[j];
           const float s = E::to_f(*reinterpret_cast<const T*>(&sraw));
+          if (FP8) {
+            // FP8: the group's fp32 partial sum of w * x, divided by the scale once
+            total += __fdiv_rn(lo, s);
+            lo = hi = cl = ch = 0.f;
+            continue;
+          }
           float z = ZSYM;
           if (ASYM) {
             constexpr int PF = 32 / BITS;
@@ -228,9 +249,9 @@ __global__ void __launch_bounds__(GEMV_MAX_WARPS * 32)
   if (nrank > 1) cluster_sync_all();  // keep peers' smem alive until rank 0 has read it
 }
 
-template <typename T, int BITS, bool ASYM, bool PERM>
+template <typename T, int BITS, bool ASYM, bool PERM, bool FP8 = false>
 static int launch_gemv_t(const MmArgs& a, int ks, int warps, int cpc) {
-  auto kern = gemv_kernel<T, BITS, ASYM, PERM>;
+  auto kern = gemv_kernel<T, BITS, ASYM, PERM, FP8>;
   if (ks > 8) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return (int)e;
@@ -271,6 +292,10 @@ int launch_gemv(const MmArgs& a) {
   if (cpc > GEMV_MAX_CPC) {
     set_error("b2q_gemv: K=%d too large for the split-K configuration (cpc=%d)", a.K, cpc);
     return -1;
+  }
+  if (a.fp8) {  // FP8 layers: e4m3 codes, no zero-points, no act-order
+    return a.dtype == 0 ? launch_gemv_t<__half, 8, false, false, true>(a, ks, warps, cpc)
+                        : launch_gemv_t<__nv_bfloat16, 8, false, false, true>(a, ks, warps, cpc);
   }
   const bool asym = a.qzeros != nullptr, perm = a.perm != nullptr;
 #define B2Q_GEMV_CASE(T, BITS)                                                        \

@@ -28,6 +28,7 @@ struct MmArgs {
   cudaStream_t stream;
   int tune_ks;     // >0: force the split-K cluster size of the M=1 GEMV and of the decode planners
   int tune_warps;  // >0: force the warps per CTA of the M=1 GEMV and of the decode planners
+  int fp8;         // 1: FP8 (e4m3fn) layer: 8-bit codes are e4m3 values, W = T(w) / T(scale) (b2q_fp8_mm)
 };
 
 // Fused row-parallel all-reduce of the decode tier (b2q_decode2.cu).  world <= 1: plain decode.
@@ -41,6 +42,8 @@ struct DecodeAR {
 int launch_decode_allreduce(const MmArgs& a, const DecodeAR& ar);
 size_t decode_allreduce_flag_bytes();
 
+int launch_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
+                       cudaStream_t stream);  // b2q_prepack.cu
 int launch_prepack(const void* qweight, const int32_t* perm, void* out, int K, int N, int bits, cudaStream_t stream);
 int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, cudaStream_t stream);
 int launch_hadamard(const void* x, const int8_t* had, int K, void* out, int rows, int n, int dtype,

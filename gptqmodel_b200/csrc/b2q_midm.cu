@@ -80,7 +80,7 @@ struct MidCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "dynamic shared memory of one CTA");
 };
 
-template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE, int DQG>
+template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE, int DQG, bool FP8 = false>
 __global__ void __launch_bounds__(MM_THREADS, 1)
     midm_kernel(const __grid_constant__ CUtensorMap tmap_x, const uint4* __restrict__ packed,
                 const T* __restrict__ scales, const uint32_t* __restrict__ qzeros, const T* __restrict__ bias,
@@ -386,10 +386,15 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
           for (int j = 0; j < 2; ++j) {
             int z = ZSYM;
             if (ASYM) z = (int)((sz[r][j].zw >> (BITS * (nsafe % PF))) & ((1u << BITS) - 1));
+            Fp8Div dv = {};
+            if constexpr (FP8) dv = fp8_div_of<T>(sz[r][j].s);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               uint4 o[2];
-              Dequant<T, 8>::run(pvs[r][j][h], sz[r][j].s, z, o);
+              if constexpr (FP8)
+                DequantFp8<T>::run(pvs[r][j][h], dv, o);
+              else
+                Dequant<T, 8>::run(pvs[r][j][h], sz[r][j].s, z, o);
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
                 const uint32_t addr = brow + (((uint32_t)(j * 4 + h * 2 + c) ^ sw) << 4);
@@ -496,13 +501,13 @@ int midm_ranks(int K, int N) {
 
 constexpr int MM_DQG = 4;  // dequant groups = k-blocks dequantised concurrently
 
-template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE = 0, int DQG = MM_DQG>
+template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE = 0, int DQG = MM_DQG, bool FP8 = false>
 static int launch_midm_t(const MmArgs& a, const void* x, int ks, const MoeArgs& G = MoeArgs{}, int x_rows = 0,
                          int grid_z = 1) {
   using C = MidCfg<BITS, NTOK, PST, WST, MODE>;
   CUtensorMap tmap;
   if (make_x_tmap_box(&tmap, x, MODE == 0 ? a.M : x_rows, a.K, a.dtype, NTOK) != 0) return -1;
-  auto kern = midm_kernel<T, BITS, ASYM, NTOK, PST, WST, MODE, DQG>;
+  auto kern = midm_kernel<T, BITS, ASYM, NTOK, PST, WST, MODE, DQG, FP8>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_midm")) return e;
   const int nkb = a.K / MM_BK;
@@ -536,7 +541,15 @@ int launch_midm(const MmArgs& a, const void* x) {
 #define B2Q_MM_CASE(T)                                                          \
   (a.bits == 4 ? (asym ? B2Q_MM_NTOK(T, 4, true) : B2Q_MM_NTOK(T, 4, false))   \
                : (asym ? B2Q_MM_NTOK(T, 8, true) : B2Q_MM_NTOK(T, 8, false)))
+  // FP8 layers: the 8-bit ring depths, no zero-points, the e4m3 / scale division in the dequant warps
+#define B2Q_MM_FP8(T)                                                                               \
+  (a.M <= 16   ? launch_midm_t<T, 8, false, 16, 8, 8, 0, MM_DQG, true>(a, x, ks)                    \
+   : a.M <= 32 ? launch_midm_t<T, 8, false, 32, 8, 8, 0, MM_DQG, true>(a, x, ks)                    \
+   : a.M <= 64 ? launch_midm_t<T, 8, false, 64, 4, 8, 0, MM_DQG, true>(a, x, ks)                    \
+               : launch_midm_t<T, 8, false, 128, 4, 8, 0, MM_DQG, true>(a, x, ks))
+  if (a.fp8) return a.dtype == 0 ? B2Q_MM_FP8(__half) : B2Q_MM_FP8(__nv_bfloat16);
   return a.dtype == 0 ? B2Q_MM_CASE(__half) : B2Q_MM_CASE(__nv_bfloat16);
+#undef B2Q_MM_FP8
 #undef B2Q_MM_CASE
 #undef B2Q_MM_NTOK
 }

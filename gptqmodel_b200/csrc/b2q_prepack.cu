@@ -6,6 +6,7 @@
 // The role of this kernel is the one gptq_marlin_repack / swordfish_prepack_B play in the reference's
 // post_init (qlinear/marlin.py:246-293, qlinear/swordfish.py:221-297): load-time only, not on the hot path.
 #include "b2q_common.cuh"
+#include "b2q_dequant.cuh"
 #include "b2q_internal.h"
 
 namespace b2q {
@@ -155,6 +156,46 @@ int launch_permute_cols(const void* x, const int32_t* perm, void* out, int M, in
   }
   dim3 grid((K + 255) / 256 > 64 ? 64 : (K + 255) / 256, M > 32768 ? 32768 : M);
   permute_cols_kernel<<<grid, 256, 0, stream>>>((const uint16_t*)x, perm, (uint16_t*)out, M, K);
+  return (int)cudaGetLastError();
+}
+
+// FP8 layers: out[k, n] = T(w[k, n]) / scales[k / group_size, n] from the prepacked T8 codes, with the same division the
+// tensor-core tiers feed the MMA (DequantFp8).  One thread per T8 uint4 (16 consecutive k of one feature); consecutive
+// lanes own consecutive features, so every store of a warp is 64 contiguous bytes.
+template <typename T>
+__global__ void fp8_dequant_kernel(const uint4* __restrict__ packed, const T* __restrict__ scales, T* __restrict__ out,
+                                   int K, int N, int group_size) {
+  const int NT = N / 32;
+  const long long total = (long long)(K / 32) * NT * 2 * 32;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int lane = (int)(idx & 31);
+  long long rest = idx >> 5;
+  const int h = (int)(rest % 2);
+  rest /= 2;
+  const int nt = (int)(rest % NT);
+  const int kc = (int)(rest / NT);
+  const int n = nt * 32 + lane, k0 = kc * 32 + h * 16;
+  const uint32_t s16 = *reinterpret_cast<const uint16_t*>(scales + (size_t)(k0 / group_size) * N + n);
+  uint4 o[2];
+  DequantFp8<T>::run(packed[idx], fp8_div_of<T>(s16), o);
+  const uint16_t* v = reinterpret_cast<const uint16_t*>(o);
+  uint16_t* dst = reinterpret_cast<uint16_t*>(out) + (size_t)k0 * N + n;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) dst[(size_t)i * N] = v[i];
+}
+
+int launch_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
+                       cudaStream_t stream) {
+  const int threads = 256;
+  const long long total = (long long)(K / 32) * (N / 32) * 2 * 32;
+  const unsigned blocks = (unsigned)((total + threads - 1) / threads);
+  if (dtype == 0)
+    fp8_dequant_kernel<__half><<<blocks, threads, 0, stream>>>((const uint4*)packed, (const __half*)scales,
+                                                               (__half*)out, K, N, group_size);
+  else
+    fp8_dequant_kernel<__nv_bfloat16><<<blocks, threads, 0, stream>>>(
+        (const uint4*)packed, (const __nv_bfloat16*)scales, (__nv_bfloat16*)out, K, N, group_size);
   return (int)cudaGetLastError();
 }
 

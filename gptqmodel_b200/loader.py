@@ -9,7 +9,8 @@ What the reference does for this step, restated for this package (no model defin
     "this module is not quantised", ``+:`` is an explicit positive match (config.py:1579-1652, 1822-1854);
   * a quantised linear ``<prefix>`` is stored as ``<prefix>.qweight / .qzeros / .scales / .g_idx [/ .bias]``
     (nn_modules/qlinear/__init__.py:827-865); AWQ GEMM checkpoints have no ``g_idx`` (:1634-1668); QQQ (W4A8)
-    checkpoints store ``<prefix>.B / .s_channel / .s_group [/ .bias]`` (nn_modules/qlinear/qqq.py);
+    checkpoints store ``<prefix>.B / .s_channel / .s_group [/ .bias]`` (nn_modules/qlinear/qqq.py); FP8 checkpoints
+    ``<prefix>.weight`` (float8_e4m3fn) ``/ .weight_scale_inv [/ .bias]`` (nn_modules/qlinear/fp8.py);
   * ``format == "gptq"`` files hold v1 zero-points (stored as zero - 1): kernels that need the true zero-point get
     ``qzeros += 0x11111111`` (4-bit) / ``0x01010101`` (8-bit) at load (utils/model.py:800-846, models/loader.py:1657-1675);
     the reference refuses asymmetric v1 files that were not produced by its own >= 0.9.0 quantiser (loader.py:1659-1663).
@@ -42,11 +43,15 @@ class QuantSpec:
     desc_act: bool = False
     sym: bool = True
     format: str = "gptq"   # "gptq" (v1 zero-points) | "gptq_v2" | "gptq_p" (planar, v2 zero-points) | "gemm" (AWQ)
-    method: str = "gptq"   # "gptq" | "awq" | "qqq"
+    method: str = "gptq"   # "gptq" | "awq" | "qqq" | "fp8"
     lm_head: bool = False
     dynamic: Optional[Dict[str, dict]] = None
     meta: dict = field(default_factory=dict)
     rotation: Optional[str] = None  # None | "hadamard" | "random": QuaRot / SpinQuant checkpoint, see load_quantized_linears
+    # FP8 checkpoints (method "fp8"): the e4m3 format and the scale layout of the reference's FP8Config
+    fp8_format: str = "float8_e4m3fn"
+    weight_scale_method: Optional[str] = None
+    weight_block_size: Optional[tuple] = None
 
     def for_module(self, name: str) -> Optional["QuantSpec"]:
         """Per-module view after `dynamic` overrides; None if a negative (`-:`) pattern excludes the module."""
@@ -59,6 +64,9 @@ class QuantSpec:
                 if negative:
                     return None
                 out = QuantSpec(**{**self.__dict__, "dynamic": None})
+                if self.method == "fp8":
+                    _fp8_override(out, name, overrides or {})
+                    return out
                 for k, v in (overrides or {}).items():
                     k = _ALIASES.get(k, k)
                     if k in ("bits", "group_size"):
@@ -94,8 +102,11 @@ def parse_quant_config(raw: dict) -> QuantSpec:
     pack_dtype = str(d.get("pack_dtype", "int32")).replace("torch.", "")
     if pack_dtype != "int32":
         raise NotImplementedError(f"pack_dtype `{pack_dtype}` is not supported (int32 words only, like Marlin / Swordfish)")
-    if spec.method not in ("gptq", "awq", "qqq"):
-        raise NotImplementedError(f"quantisation method `{spec.method}` is outside this package (gptq, awq, qqq)")
+    if spec.method not in ("gptq", "awq", "qqq", "fp8"):
+        raise NotImplementedError(f"quantisation method `{spec.method}` is outside this package (gptq, awq, qqq, fp8)")
+    if spec.method == "fp8":
+        _parse_fp8(spec, raw)
+        return spec
     if spec.method == "qqq":
         if fmt is None:
             spec.format = "qqq"
@@ -122,6 +133,58 @@ def _check_qqq(spec: QuantSpec) -> None:
                                   "(4-bit, group size -1 or 128, symmetric)")
     if spec.rotation is not None:
         raise NotImplementedError("`rotation` is not supported for QQQ checkpoints")
+
+
+def _parse_fp8(spec: QuantSpec, raw: dict) -> None:
+    """FP8 configs as the reference's FP8Config writes them: `format` (or the legacy `fmt`) names the e4m3 dtype,
+    `weight_scale_method` / `weight_block_size` / `weight_scale_semantics` the scales, group size and act-order do not
+    apply.  HF / DeepSeek-native FP8 configs (`activation_scheme`, or `fmt` without `format`) store a `weight_scale_inv`
+    that MULTIPLIES the weights; serving them with this package's division would give wrong outputs, so they are refused."""
+    from .fp8 import normalize_block_size, normalize_fp8_format, normalize_scale_method, normalize_scale_semantics
+
+    if "activation_scheme" in raw or ("fmt" in raw and "format" not in raw):
+        raise NotImplementedError("HF / DeepSeek-native FP8 checkpoints (weight_scale_inv as a multiplier) are not "
+                                  "supported; only the reference's FP8Config (weight = w / weight_scale_inv) is")
+    if raw.get("rotation"):
+        raise NotImplementedError("`rotation` is not supported for FP8 checkpoints")
+    if int(raw.get("bits", 8)) != 8:
+        raise ValueError("FP8: `bits` must be 8")
+    fmt = raw.get("format", raw.get("fmt"))
+    spec.fp8_format = normalize_fp8_format(fmt)
+    spec.format = "fp8"
+    spec.bits, spec.group_size, spec.desc_act, spec.sym = 8, -1, False, True
+    spec.weight_block_size = normalize_block_size(raw.get("weight_block_size"))
+    spec.weight_scale_method = normalize_scale_method(raw.get("weight_scale_method"), spec.weight_block_size)
+    normalize_scale_semantics(raw.get("weight_scale_semantics"))
+    for layer, overrides in (spec.dynamic or {}).items():
+        if not layer.startswith("-:"):
+            _fp8_override(QuantSpec(**{**spec.__dict__, "dynamic": None}), layer, overrides or {})
+
+
+def _fp8_override(out: QuantSpec, name: str, overrides: dict) -> None:
+    """Apply one `dynamic` entry of an FP8 config (the reference's per-layer rules) to a module's spec."""
+    from .fp8 import normalize_block_size, normalize_fp8_format, normalize_scale_method, normalize_scale_semantics
+
+    if "bits" in overrides and int(overrides["bits"]) != 8:
+        raise ValueError(f"FP8: layer `{name}` only supports 8-bit FP8 weights")
+    if overrides.get("group_size") not in (-1, None):
+        raise ValueError("FP8: `group_size` is not used; keep it at `-1`")
+    fmt = overrides.get("format", overrides.get("fmt"))
+    if fmt is not None:
+        out.fp8_format = normalize_fp8_format(fmt)
+    block = normalize_block_size(overrides.get("weight_block_size"))
+    if "weight_scale_method" in overrides or block is not None:
+        out.weight_scale_method = normalize_scale_method(overrides.get("weight_scale_method"), block)
+        out.weight_block_size = block
+    if "weight_scale_semantics" in overrides:
+        normalize_scale_semantics(overrides["weight_scale_semantics"])
+
+
+def fp8_prefixes(names: Iterable[str]) -> list:
+    """Module prefixes of an FP8 checkpoint (`<prefix>.weight_scale_inv` together with `<prefix>.weight`)."""
+    names = set(names)
+    sfx = ".weight_scale_inv"
+    return sorted(n[: -len(sfx)] for n in names if n.endswith(sfx) and n[: -len(sfx)] + ".weight" in names)
 
 
 def read_quant_config(path: str) -> QuantSpec:
@@ -238,6 +301,7 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
     from safetensors import safe_open
 
     from .awq import B200AwqQuantLinear
+    from .fp8 import B200Fp8QuantLinear
     from .qlinear import B200QuantLinear
     from .qqq import B200QqqQuantLinear
 
@@ -246,7 +310,7 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
     if only is not None:
         prefixes = list(only)
     else:
-        prefixes = qqq_prefixes(wmap) if spec.method == "qqq" else quantized_prefixes(wmap)
+        prefixes = {"qqq": qqq_prefixes, "fp8": fp8_prefixes}.get(spec.method, quantized_prefixes)(wmap)
     dev = torch.device(device)
     do_post = (dev.type == "cuda") if post_init is None else post_init
     handles: Dict[str, object] = {}
@@ -265,6 +329,22 @@ def load_quantized_linears(path: str, device="cuda", dtype: Optional[torch.dtype
             ms = spec.for_module(prefix)
             if ms is None:
                 continue  # excluded by a negative dynamic pattern: stays a dense layer in the model
+            if ms.method == "fp8":
+                t = {s: tensor(f"{prefix}.{s}") for s in ("weight", "weight_scale_inv", "weight_scale", "bias")}
+                if t["weight"] is None or t["weight_scale_inv"] is None:
+                    if t["weight_scale"] is not None:
+                        raise NotImplementedError(f"{prefix}: ModelOpt-style FP8 tensors (`weight_scale` without "
+                                                  "`weight_scale_inv`) are not supported")
+                    raise KeyError(f"{prefix}: checkpoint misses weight / weight_scale_inv")
+                if t["weight"].dtype != torch.float8_e4m3fn:
+                    raise NotImplementedError(f"{prefix}: weight dtype {t['weight'].dtype} is not served "
+                                              "(float8_e4m3fn only)")
+                m = B200Fp8QuantLinear.from_checkpoint_tensors(
+                    t["weight"], t["weight_scale_inv"], bias=t["bias"], weight_scale_method=ms.weight_scale_method,
+                    weight_block_size=ms.weight_block_size, format=ms.fp8_format, device=dev, dtype=dtype,
+                    post_init=do_post, name=prefix)
+                mods[prefix] = m
+                continue
             if ms.method == "qqq":
                 _check_qqq(ms)  # a `dynamic` override may have changed bits / group size
                 t = {s: tensor(f"{prefix}.{s}") for s in ("B", "s_channel", "s_group", "bias")}

@@ -23,6 +23,8 @@ Layer = Dict[str, object]
 
 
 def _check(layer: Layer):
+    if "weight_scale_inv" in layer:
+        raise NotImplementedError("tensor parallelism of FP8 layers is not supported")
     for k in ("qweight", "qzeros", "scales", "g_idx", "bits", "group_size"):
         if k not in layer:
             raise KeyError(f"layer dict misses {k!r}")
@@ -244,6 +246,8 @@ class RowParallelLinear(torch.nn.Module):
         if getattr(inner, "online_full_had", False) or getattr(inner, "online_partial_had", False):
             # the online Hadamard transform mixes all K input columns; a row shard holds K / world of them
             raise NotImplementedError("RowParallelLinear: rotated layers (online Hadamard transform) cannot be row-sharded")
+        if getattr(inner, "QUANT_TYPE", None) == "b200_fp8":
+            raise NotImplementedError("RowParallelLinear: tensor parallelism of FP8 layers is not supported")
         super().__init__()
         self.inner = inner
         self.group = group

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B2Q_ABI_VERSION 7
+#define B2Q_ABI_VERSION 8
 #define B2Q_DTYPE_F16 0
 #define B2Q_DTYPE_BF16 1
 
@@ -233,6 +233,24 @@ int b2q_qqq_mm(const int8_t* q, const float* s_tok, const void* packed, const fl
 int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, const void* s_group, const void* bias,
                     void* out, int M, int K, int N, int group_size, int dtype, int out_dtype, void* workspace,
                     size_t workspace_bytes, void* stream);
+
+/* FP8 (e4m3fn, W8A16) layers on the 8-bit tiers (ABI v8).  The arithmetic of the reference's TorchFP8Linear
+ * (gptqmodel/nn_modules/qlinear/fp8.py, its dequantise-then-matmul path), T = fp16 (dtype 0) or bf16 (dtype 1):
+ *   W[k, n] = RN_T( float(T(w[n, k])) / float(scales[k / group_size, n]) )      (correctly rounded division)
+ *   out     = T(x @ W) (fp32 accumulation), then T(out + bias)
+ * The M > 1 tiers feed the tensor cores exactly that W; the M = 1 GEMV (K % 128 == 0) sums w * x of a group in fp32 and
+ * divides the sum by the scale once.
+ *   packed : b2q_prepack(bits = 8) of the codes packed like an 8-bit GPTQ qweight (int32 [K/4, N], code of row 4i+j in
+ *            byte j of word [i, n]); the byte is the e4m3fn bit pattern
+ *   scales : T [K / group_size, N], scale_inv rounded to T and expanded over the output rows of its block;
+ *            group_size 64 | 128 (dividing K) or K (per-channel and per-tensor layers)
+ *   x, out: T, [M, K] / [M, N] contiguous, 16-byte aligned; bias T [N] or NULL; workspace unused (may be NULL)
+ * Dispatches on M inside the library, so a CUDA graph sees the true M.  K % 64 == 0, N % 32 == 0. */
+int b2q_fp8_mm(const void* x, const void* packed, const void* scales, const void* bias, void* out, int M, int K, int N,
+               int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream);
+/* out[K, N] (T, row-major) = W of b2q_fp8_mm, exactly the operand the tensor-core tiers multiply. */
+int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
+                    void* stream);
 
 #ifdef __cplusplus
 }
