@@ -170,6 +170,23 @@ int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, i
   return 0;
 }
 
+int b2q_debug_decode_occupancy(int version, int M, int K, int N, int ks, int warps, int* blocks) {
+  if (blocks == nullptr || (version != 1 && version != 2) || M < 1 || M > 8 || K < 128 || K % 128 != 0 || N < 32 ||
+      N % 32 != 0) {
+    set_error("b2q_debug_decode_occupancy: bad argument (version=%d M=%d K=%d N=%d)", version, M, K, N);
+    return -2;
+  }
+  MmArgs a = {};
+  a.M = M;
+  a.K = K;
+  a.N = N;
+  a.bits = 4;
+  a.group_size = 128;
+  a.tune_ks = ks;
+  a.tune_warps = warps;
+  return decode_occupancy(version, a, N / 32, blocks);
+}
+
 const char* b2q_last_error(void) { return g_err; }
 
 size_t b2q_packed_bytes(int K, int N, int bits) { return (size_t)K * (size_t)N * (size_t)bits / 8; }

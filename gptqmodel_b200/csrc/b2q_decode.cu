@@ -13,8 +13,8 @@
 //    which is algebraically the reference's  s * (q - z)  applied inside the sum (qlinear/__init__.py:1001-1003);
 //  * grid = (N/32 feature tiles) x (KS split-K CTAs in a thread-block cluster); partial sums are reduced through
 //    distributed shared memory (no atomics, no workspace, no output zeroing, deterministic);
-//  * every lane issues its 4 x LDG.128 of weights (+ scales) BEFORE griddepcontrol.wait (programmatic dependent
-//    launch): weights never depend on the previous kernel, so consecutive layers overlap their HBM streams;
+//  * each warp's first ring stages (weights + their scales, b2q_decode.cuh issue_quad) are requested BEFORE
+//    griddepcontrol.wait (programmatic dependent launch): weights never depend on the previous kernel;
 //  * act-order: rows sorted by group at prepack; the activation staging reads x and the INVERSE permutation coalesced
 //    and scatters into shared memory (stage_x_act_order, b2q_decode.cuh).
 // Replaces the decode tiers of swordfish_mm (swordfish_mm.cu:216-286, mma.sync + cp.async + atomics) and Marlin's
@@ -36,7 +36,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   // ahead of the PDL wait — the wait moves to the top (the later one is then a no-op)
   if (MOE) asm volatile("griddepcontrol.wait;" ::: "memory");
   // dynamic smem: ring[nwarps][DEC_STAGES][2 KB] | sx[M][kspan] (T) | xsum[kblocks][8] | red[2][nwarps][8][32] |
-  //               part[max_tiles][8][32] | mbarriers[nwarps][DEC_STAGES]
+  //               part[max_tiles][8][32] | mbarriers[nwarps][DEC_STAGES] | scale slots[nwarps][nst][SCB]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int g = lane >> 2, t = lane & 3;
   // The CTA walks tiles tile0, tile0 + C, ...; all `gw` warps split the k-quads of every tile (wg = warp's index).
@@ -58,6 +58,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   float* red = xsum + qpc * 2 * 8;
   float* part = red + 2 * nwarps * 256;  // [max_tiles][256]
   const uint32_t bars = smem_u32(part + max_tiles * 256) + warp * DEC_STAGES * 8;
+  constexpr int NG = G64 ? 2 : 1, SCB = dec_sc_bytes(ASYM, G64);
+  const uint32_t sring_w = smem_u32(part + max_tiles * 256) + nwarps * DEC_STAGES * 8 + warp * nst * SCB;
   const bool PERM = perm != nullptr;
 
   // ---- 1. the first DEC_STAGES quads of this warp requested before anything else -----------------
@@ -65,16 +67,25 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   const int U = ntiles * nq;                                                     // units of this warp
   // issue cursor (lane 0): quads of a tile are 2*nwarps k-blocks apart; the tile -> (weight set, local tile) mapping is
   // resolved once per tile
+  // quantisation groups between consecutive quads of this warp, and the group of its first quad in every tile
+  const int gstep = (2 * gw) >> gsh;
+  const int g_first = (2 * (q0 + wg)) >> gsh;
   const uint4* iss_src = nullptr;
+  const T* iss_sc = nullptr;          // scale row of the next quad to issue (features of its tile)
+  const uint32_t* iss_zq = nullptr;   // qzeros row of the same
+  int iss_N = 0;
   size_t iss_kbs = 0;  // k-block stride (uint4) of the set being issued
   int iss_q = 0, iss_u = 0, iss_ti = 0;
   auto iss_begin_tile = [&]() {
     const TileRef<T> r = resolve_tile<T, MOE>(S, tile0 + iss_ti * C);
     iss_kbs = (size_t)(r.N >> 4) * 32;
     iss_src = r.w + (size_t)(2 * (q0 + wg)) * iss_kbs + (size_t)(2 * r.nt) * 32;
+    iss_N = r.N;
+    iss_sc = r.sc + (size_t)g_first * r.N + r.nt * 32;
+    if (ASYM) iss_zq = r.zq + (size_t)g_first * (r.N >> 3) + r.nt * 4;
   };
-  auto iss_one = [&](uint32_t dst, uint32_t bar) {
-    issue_quad(dst, bar, iss_src, iss_kbs);
+  auto iss_one = [&](uint32_t dst, uint32_t sdst, uint32_t bar) {
+    issue_quad<T, ASYM, G64>(dst, sdst, bar, iss_src, iss_kbs, iss_sc, iss_zq, iss_N);
     ++iss_u;
     if (++iss_q == nq) {
       iss_q = 0;
@@ -82,6 +93,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
       if (iss_u < U) iss_begin_tile();
     } else {
       iss_src += (size_t)(2 * gw) * iss_kbs;
+      iss_sc += (size_t)gstep * iss_N;
+      if (ASYM) iss_zq += (size_t)gstep * (iss_N >> 3);
     }
   };
   if (lane == 0) {
@@ -91,48 +104,9 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     if (U > 0) iss_begin_tile();
 #pragma unroll
     for (int i = 0; i < DEC_STAGES; ++i)
-      if (i < nst && iss_u < U) iss_one(smem_u32(ring) + i * DEC_QUAD_BYTES, bars + 8 * i);
+      if (i < nst && iss_u < U) iss_one(smem_u32(ring) + i * DEC_QUAD_BYTES, sring_w + i * SCB, bars + 8 * i);
   }
   // scale / zero prefetch cursor (all lanes): this lane's 4 feature rows are +0, +8, +16, +24 from sc_next
-  const int gstep = (2 * gw) >> gsh;           // quantisation groups between consecutive quads of this warp
-  const int g_first = (2 * (q0 + wg)) >> gsh;  // quantisation group of this warp's first quad in every tile
-  const T* sc_next = nullptr;
-  const uint32_t* zq_next = nullptr;
-  int pre_q = 0, pre_ti = 0, pre_N = 0;
-  auto pre_begin_tile = [&]() {
-    const TileRef<T> r = resolve_tile<T, MOE>(S, tile0 + pre_ti * C);
-    pre_N = r.N;
-    sc_next = r.sc + (size_t)g_first * r.N + r.nt * 32 + g;
-    if (ASYM) zq_next = r.zq + (size_t)g_first * (r.N >> 3) + r.nt * 4;
-  };
-  auto fetch_scales = [&](DScale<ASYM, G64>& d) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      d.s[0][i] = *reinterpret_cast<const uint16_t*>(sc_next + i * 8);
-      if (ASYM) d.zw[0][i] = zq_next[i];
-    }
-    if (G64) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        d.s[G64 ? 1 : 0][i] = *reinterpret_cast<const uint16_t*>(sc_next + (size_t)pre_N + i * 8);
-        if (ASYM) d.zw[G64 ? 1 : 0][i] = zq_next[(pre_N >> 3) + i];
-      }
-    }
-    // advance to the next unit
-    if (++pre_q == nq) {
-      pre_q = 0;
-      ++pre_ti;
-      if (pre_ti < ntiles) pre_begin_tile();
-    } else {
-      sc_next += (size_t)gstep * pre_N;
-      if (ASYM) zq_next += (size_t)gstep * (pre_N >> 3);
-    }
-  };
-  DScale<ASYM, G64> cur;
-  if (U > 0) {
-    pre_begin_tile();
-    fetch_scales(cur);
-  }
 
   if (PERM) prefetch_inverse_perm(perm + K, K);
   // zero the token columns >= M of the block sums once (read by the fix-up of lanes whose columns are padding): own shared
@@ -185,11 +159,10 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
 
     uint32_t xf_a = xf_a0, xs_a = xs_a0;
     for (int qi = 0; qi < nq; ++qi, ++u, xf_a += xf_qstep, xs_a += xs_qstep) {
-      DScale<ASYM, G64> nxt;
-      if (u + 1 < U) fetch_scales(nxt);
       const int st = u & (nst - 1);
       mbar_wait(bars + 8 * st, (uint32_t)(u >> stl) & 1u);
       const uint32_t wq_a = ring_a + st * DEC_QUAD_BYTES;
+      const uint32_t sc_a = sring_w + st * SCB;  // this quad's scales / zeros (complete with the stage's barrier)
       float dd[2][2][4];  // [kbl][ftl][c]: four independent mma accumulator chains
 #pragma unroll
       for (int a = 0; a < 2; ++a)
@@ -229,13 +202,14 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
           const int gi = G64 ? kbl : 0;  // compile-time after unrolling
 #pragma unroll
           for (int ftl = 0; ftl < 2; ++ftl) {
-            const uint16_t slr = cur.s[gi][ftl * 2], shr = cur.s[gi][ftl * 2 + 1];
+            const uint16_t slr = lds_u16(sc_a + gi * 64 + (ftl * 16 + g) * 2);
+            const uint16_t shr = lds_u16(sc_a + gi * 64 + (ftl * 16 + g + 8) * 2);
             const float sl = E::to_f(*reinterpret_cast<const T*>(&slr));
             const float sh = E::to_f(*reinterpret_cast<const T*>(&shr));
             float zl = ZSYM, zh = ZSYM;
             if (ASYM) {
-              zl = (float)((cur.zw[ASYM ? gi : 0][ftl * 2] >> (4 * g)) & 15u);  // feature % 8 == g for all rows
-              zh = (float)((cur.zw[ASYM ? gi : 0][ftl * 2 + 1] >> (4 * g)) & 15u);
+              zl = (float)((lds_u32(sc_a + NG * 64 + gi * 16 + ftl * 8) >> (4 * g)) & 15u);  // feature % 8 == g for all rows
+              zh = (float)((lds_u32(sc_a + NG * 64 + gi * 16 + ftl * 8 + 4) >> (4 * g)) & 15u);
             }
             const float bl = E::LO_BASE + zl, bh = E::HI_BASE + zh;
             float d[4];
@@ -251,8 +225,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
       }
       // recycle the stage for the next not-yet-issued unit (all lanes have finished reading it)
       __syncwarp();
-      if (lane == 0 && iss_u < U) iss_one(ring_a + st * DEC_QUAD_BYTES, bars + 8 * st);
-      if (u + 1 < U) cur = nxt;
+      if (lane == 0 && iss_u < U) iss_one(ring_a + st * DEC_QUAD_BYTES, sring_w + st * SCB, bars + 8 * st);
     }
 
     // ---- tile epilogue: warps -> CTA through (double-buffered) smem, one barrier per tile ---------
@@ -365,9 +338,11 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   }
 }
 
-static size_t decode_smem(int M, int warps, int qpc, int max_tiles, int nst) {
-  return (size_t)warps * nst * DEC_QUAD_BYTES + (size_t)M * qpc * 128 * 2 + (size_t)qpc * 2 * 8 * 4 +
-         (size_t)2 * warps * 256 * 4 + (size_t)max_tiles * 256 * 4 + (size_t)warps * DEC_STAGES * 8 + 16;
+static size_t decode_smem(const MmArgs& a, int warps, int qpc, int max_tiles, int nst) {
+  const int scb = dec_sc_bytes(a.qzeros != nullptr, a.group_size == 64);
+  return (size_t)warps * nst * DEC_QUAD_BYTES + (size_t)a.M * qpc * 128 * 2 + (size_t)qpc * 2 * 8 * 4 +
+         (size_t)2 * warps * 256 * 4 + (size_t)max_tiles * 256 * 4 + (size_t)warps * DEC_STAGES * 8 +
+         (size_t)warps * nst * scb + 16;
 }
 
 // Pick (C tile-columns, ks split-K ranks, warps) minimising the critical path in "quads per warp" on one CTA per SM.
@@ -387,7 +362,7 @@ static bool decode_config(const MmArgs& a, int NT, DecodePlan& best) {
       if (C < 1) C = 1;
       const int max_tiles = (NT + C - 1) / C;
       DecodePlan p = {C, ks, warps, warps, qpc, ks > 1 ? max_tiles : 0, 0, 0};
-      if (!fit_ring(p, [&](int nst) { return decode_smem(a.M, warps, qpc, p.max_tiles, nst); })) continue;
+      if (!fit_ring(p, [&](int nst) { return decode_smem(a, warps, qpc, p.max_tiles, nst); })) continue;
       const int qpw = (qpc + warps - 1) / warps;  // quads per warp per tile
       // relative cost in units of one quad per warp: per tile = quads/warp + barrier epilogue, split-K adds a cluster
       // barrier + DSMEM pass, fewer warps hide less latency (the weights are heuristic, not fitted to one GPU)
@@ -413,6 +388,19 @@ bool decode_plan(int version, const MmArgs& a, int NT, int* out8) {
   return true;
 }
 
+int decode2_occupancy(const DecodePlan& c, int* blocks);  // b2q_decode2.cu
+
+int decode_occupancy(int version, const MmArgs& a, int NT, int* blocks) {
+  DecodePlan c;
+  if (!(version == 2 ? decode2_config(a, NT, c) : decode_config(a, NT, c))) {
+    set_error("b2q_debug_decode_occupancy: no configuration fits shared memory (version=%d M=%d K=%d N=%d)", version,
+              a.M, a.K, a.N);
+    return -1;
+  }
+  if (version == 2) return decode2_occupancy(c, blocks);
+  return plan_occupancy(decode_kernel<__half, false, false, false>, c, blocks);
+}
+
 template <typename I>
 static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodePlan& c, const DecodeAR& ar) {
   using T = typename I::T;
@@ -424,6 +412,7 @@ static int launch_decode_t(const MmArgs& a, const DecSets& sets, const DecodePla
 }
 
 static int launch_decode_plan(const MmArgs& a, const DecSets& sets, const DecodePlan& c, const DecodeAR& ar) {
+  if (!sets_aligned(sets, "b2q_decode")) return -1;
   return dispatch_decode(a, sets, [&](auto inst) { return launch_decode_t<decltype(inst)>(a, sets, c, ar); });
 }
 
@@ -585,7 +574,7 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
   c.C = num_sms() / top_k;
   if (c.C > NT) c.C = NT;
   c.max_tiles = (NT + c.C - 1) / c.C;
-  if (!fit_ring(c, [&](int nst) { return decode_smem(1, c.warps, c.qpc, c.max_tiles, nst); })) {
+  if (!fit_ring(c, [&](int nst) { return decode_smem(a, c.warps, c.qpc, c.max_tiles, nst); })) {
     set_error("b2q_moe_decode_down: K=%d does not fit shared memory", a.K);
     return -1;
   }

@@ -1,5 +1,5 @@
 // b2q_decode.cuh — definitions shared by the decode-tier kernels (b2q_decode.cu, b2q_decode2.cu): the per-warp
-// cp.async.bulk ring geometry, the mma.sync wrapper, the per-unit scale / zero registers and the multi-set ("sibling"
+// cp.async.bulk ring geometry (weights and their scale / zero slots), the mma.sync wrapper and the multi-set ("sibling"
 // QuantLinears) tile index space; on the host, the launch plan and the kernel dispatch of both.
 #pragma once
 #include "b2q_common.cuh"
@@ -35,11 +35,12 @@ __device__ __forceinline__ void mma_16816<__nv_bfloat16>(float (&d)[4], const ui
 constexpr int DEC_STAGES = 4;  // maximum ring depth; the launch picks 4 or 2 stages (`stl` = log2) to fit shared memory
 constexpr int DEC_QUAD_BYTES = 2048;
 
-template <bool ASYM, bool G64>
-struct DScale {
-  uint16_t s[G64 ? 2 : 1][4];  // [group in quad][ftl * 2 + hi]
-  uint32_t zw[(ASYM ? 1 : 0) * (G64 ? 2 : 1) + (ASYM ? 0 : 1)][4];
-};
+// The scales (and zero points) of a quad travel in the same ring stage as its weights: one cp.async.bulk per group row
+// of the quad's 32 features (64 B of scales, 16 B of packed zeros) into a per-stage slot of dec_sc_bytes, completing on
+// the stage's mbarrier.  They are then as far ahead of the main loop as the weights — fetched one quad ahead in
+// registers, every quad waited a full HBM round trip for its scales while 3 of 4 weight stages sat ready.
+// slot: scales[group in quad][32] (T) | zeros[group in quad][4] (u32, ASYM only)
+__host__ __device__ constexpr int dec_sc_bytes(bool asym, bool g64) { return (g64 ? 2 : 1) * (64 + (asym ? 16 : 0)); }
 
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
   uint4 r;
@@ -52,11 +53,32 @@ __device__ __forceinline__ float2 lds_f2(uint32_t a) {
   return r;
 }
 
-__device__ __forceinline__ void issue_quad(uint32_t dst, uint32_t bar, const uint4* __restrict__ src,
-                                           size_t kb_stride) {
-  mbar_expect_tx(bar, DEC_QUAD_BYTES);
+__device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
+  uint32_t r;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a));
+  return r;
+}
+__device__ __forceinline__ uint16_t lds_u16(uint32_t a) {
+  uint16_t r;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(r) : "r"(a));
+  return r;
+}
+
+// One ring stage: the quad's weights into dst, its scales / zeros (rows sc, zq of the scale / qzeros tensors, N features
+// per row) into the slot sdst.
+template <typename T, bool ASYM, bool G64>
+__device__ __forceinline__ void issue_quad(uint32_t dst, uint32_t sdst, uint32_t bar, const uint4* __restrict__ src,
+                                           size_t kb_stride, const T* sc, const uint32_t* zq, int N) {
+  constexpr int NG = G64 ? 2 : 1;
+  mbar_expect_tx(bar, DEC_QUAD_BYTES + dec_sc_bytes(ASYM, G64));
   bulk_load(dst, src, 1024, bar);                     // k-block 2q   : feature tiles 2nt, 2nt+1
   bulk_load(dst + 1024, src + kb_stride, 1024, bar);  // k-block 2q+1
+  bulk_load(sdst, sc, 64, bar);
+  if (G64) bulk_load(sdst + 64, sc + N, 64, bar);
+  if (ASYM) {
+    bulk_load(sdst + NG * 64, zq, 16, bar);
+    if (G64) bulk_load(sdst + NG * 64 + 16, zq + (N >> 3), 16, bar);
+  }
 }
 
 // Persistent-style CTA: blockIdx.x strides over the 32-feature tiles (tile = blockIdx.x + i * gridDim.x), blockIdx.y is
@@ -350,6 +372,27 @@ inline bool fit_ring(DecodePlan& p, SmemOf smem_of) {
 }
 
 bool decode2_config(const MmArgs& a, int NT, DecodePlan& best);  // b2q_decode2.cu
+
+// Resident CTAs per SM of a decode kernel at plan c (b2q_debug_decode_occupancy).  The opt-in is the device's maximum,
+// never below what a launch of the same kernel has opted in to.
+template <typename Kern>
+inline int plan_occupancy(Kern kern, const DecodePlan& c, int* blocks) {
+  int dev = 0, optin = 0;
+  cudaGetDevice(&dev);
+  if (int e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) return e;
+  if (int e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, optin)) return e;
+  return (int)cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks, kern, c.warps * 32, c.smem);
+}
+
+// The scale / qzeros rows are bulk-copied (issue_quad): their tensors must be 16-byte aligned (every row then is).
+inline bool sets_aligned(const DecSets& s, const char* who) {
+  for (int i = 0; i < DEC_MAX_SETS; ++i)
+    if ((reinterpret_cast<uintptr_t>(s.scales[i]) | reinterpret_cast<uintptr_t>(s.qzeros[i])) & 15u) {
+      set_error("%s: scales / qzeros of set %d are not 16-byte aligned", who, i);
+      return false;
+    }
+  return true;
+}
 
 // log2(64-k blocks per quantisation group) of the decode kernels; 31 = per-channel (every k-block is group 0)
 inline int decode_gsh(int group_size) { return group_size == 64 ? 0 : group_size == 128 ? 1 : 31; }

@@ -47,7 +47,7 @@ __device__ __forceinline__ uint32_t dec_ld_acquire_sys(const uint32_t* p) {
 // symmetric buffer: f32 data[2][world][max_elems] | (at flag_offset) u32 flags[world][DEC_AR_MAXCTA]
 // dynamic smem: ring[nwarps][nst][2 KB] | sx[M][kspan] (T) | xsum[qpc * 2][8] f32 |
 //               wpart[ngroups][max_tiles][M][gw][32] f32 | cpart[ngroups][max_tiles][M][32] f32 (split-K only) |
-//               mbarriers[nwarps][DEC_STAGES] + 1 (activations)
+//               mbarriers[nwarps][DEC_STAGES] + 1 (activations) | 8 B pad | scale slots[nwarps][nst][SCB]
 template <typename T, bool ASYM, bool G64, bool MOE>
 __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     decode2_kernel(const __grid_constant__ DecSets S, const int32_t* __restrict__ perm, const T* __restrict__ x, int M,
@@ -80,22 +80,33 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   const uint32_t bars0 = smem_u32(cpart + (nrank > 1 ? (size_t)rows * 32 : 0));
   const uint32_t bars = bars0 + warp * DEC_STAGES * 8;
   const uint32_t xbar = bars0 + nwarps * DEC_STAGES * 8;
+  constexpr int NG = G64 ? 2 : 1, SCB = dec_sc_bytes(ASYM, G64);
+  const uint32_t sring_w = xbar + 16 + warp * nst * SCB;
   const bool PERM = perm != nullptr;
   const bool XTMA = (xtma & 1) != 0 && !PERM;  // bulk-copied activations (B2Q_DECODE2_XTMA=1)
 
   // ---- 1. the first ring stages of this warp requested before anything else -------------------------
   const int nq = (q0 + wg < q1) ? (q1 - q0 - wg + gw - 1) / gw : 0;  // quads per tile for this warp
   const int U = ntiles * nq;                                         // units (quads) of this warp
+  // quantisation groups between consecutive quads of this warp, and the group of its first quad in every tile
+  const int gstep = (2 * gw) >> gsh;
+  const int g_first = (2 * (q0 + wg)) >> gsh;
   const uint4* iss_src = nullptr;
+  const T* iss_sc = nullptr;          // scale row of the next quad to issue (features of its tile)
+  const uint32_t* iss_zq = nullptr;   // qzeros row of the same
+  int iss_N = 0;
   size_t iss_kbs = 0;
   int iss_q = 0, iss_u = 0, iss_ti = 0;
   auto iss_begin_tile = [&]() {
     const TileRef<T> r = resolve_tile<T, MOE>(S, tile0 + iss_ti * C);
     iss_kbs = (size_t)(r.N >> 4) * 32;
     iss_src = r.w + (size_t)(2 * (q0 + wg)) * iss_kbs + (size_t)(2 * r.nt) * 32;
+    iss_N = r.N;
+    iss_sc = r.sc + (size_t)g_first * r.N + r.nt * 32;
+    if (ASYM) iss_zq = r.zq + (size_t)g_first * (r.N >> 3) + r.nt * 4;
   };
-  auto iss_one = [&](uint32_t dst, uint32_t bar) {
-    issue_quad(dst, bar, iss_src, iss_kbs);
+  auto iss_one = [&](uint32_t dst, uint32_t sdst, uint32_t bar) {
+    issue_quad<T, ASYM, G64>(dst, sdst, bar, iss_src, iss_kbs, iss_sc, iss_zq, iss_N);
     ++iss_u;
     if (++iss_q == nq) {
       iss_q = 0;
@@ -103,6 +114,8 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
       if (iss_u < U) iss_begin_tile();
     } else {
       iss_src += (size_t)(2 * gw) * iss_kbs;
+      iss_sc += (size_t)gstep * iss_N;
+      if (ASYM) iss_zq += (size_t)gstep * (iss_N >> 3);
     }
   };
   if (lane == 0) {
@@ -113,45 +126,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
     if (U > 0) iss_begin_tile();
 #pragma unroll
     for (int i = 0; i < DEC_STAGES; ++i)
-      if (i < nst && iss_u < U) iss_one(smem_u32(ring) + i * DEC_QUAD_BYTES, bars + 8 * i);
-  }
-  const int gstep = (2 * gw) >> gsh;
-  const int g_first = (2 * (q0 + wg)) >> gsh;
-  const T* sc_next = nullptr;
-  const uint32_t* zq_next = nullptr;
-  int pre_q = 0, pre_ti = 0, pre_N = 0;
-  auto pre_begin_tile = [&]() {
-    const TileRef<T> r = resolve_tile<T, MOE>(S, tile0 + pre_ti * C);
-    pre_N = r.N;
-    sc_next = r.sc + (size_t)g_first * r.N + r.nt * 32 + g;
-    if (ASYM) zq_next = r.zq + (size_t)g_first * (r.N >> 3) + r.nt * 4;
-  };
-  auto fetch_scales = [&](DScale<ASYM, G64>& d) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      d.s[0][i] = *reinterpret_cast<const uint16_t*>(sc_next + i * 8);
-      if (ASYM) d.zw[0][i] = zq_next[i];
-    }
-    if (G64) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        d.s[G64 ? 1 : 0][i] = *reinterpret_cast<const uint16_t*>(sc_next + (size_t)pre_N + i * 8);
-        if (ASYM) d.zw[G64 ? 1 : 0][i] = zq_next[(pre_N >> 3) + i];
-      }
-    }
-    if (++pre_q == nq) {
-      pre_q = 0;
-      ++pre_ti;
-      if (pre_ti < ntiles) pre_begin_tile();
-    } else {
-      sc_next += (size_t)gstep * pre_N;
-      if (ASYM) zq_next += (size_t)gstep * (pre_N >> 3);
-    }
-  };
-  DScale<ASYM, G64> cur;
-  if (U > 0) {
-    pre_begin_tile();
-    fetch_scales(cur);
+      if (i < nst && iss_u < U) iss_one(smem_u32(ring) + i * DEC_QUAD_BYTES, sring_w + i * SCB, bars + 8 * i);
   }
   // every warp's mbarriers (and the activation barrier) are initialised before anybody polls them; this barrier sits
   // in the part of the kernel that overlaps the previous layer (PDL), so it is free
@@ -253,11 +228,10 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
 
     uint32_t xf_a = xf_a0, xs_a = xs_a0;
     for (int qi = 0; qi < nq; ++qi, ++u, xf_a += xf_qstep, xs_a += xs_qstep) {
-      DScale<ASYM, G64> nxt;
-      if (u + 1 < U) fetch_scales(nxt);
       const int st = u & (nst - 1);
       mbar_wait(bars + 8 * st, (uint32_t)(u >> stl) & 1u);
       const uint32_t wq_a = ring_a + st * DEC_QUAD_BYTES;
+      const uint32_t sc_a = sring_w + st * SCB;  // this quad's scales / zeros (complete with the stage's barrier)
       float dd[2][2][4];  // [kbl][ftl][c]: four independent mma accumulator chains
 #pragma unroll
       for (int a = 0; a < 2; ++a)
@@ -295,13 +269,14 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
           const int gi = G64 ? kbl : 0;
 #pragma unroll
           for (int ftl = 0; ftl < 2; ++ftl) {
-            const uint16_t slr = cur.s[gi][ftl * 2], shr = cur.s[gi][ftl * 2 + 1];
+            const uint16_t slr = lds_u16(sc_a + gi * 64 + (ftl * 16 + g) * 2);
+            const uint16_t shr = lds_u16(sc_a + gi * 64 + (ftl * 16 + g + 8) * 2);
             const float sl = E::to_f(*reinterpret_cast<const T*>(&slr));
             const float sh = E::to_f(*reinterpret_cast<const T*>(&shr));
             float zl = ZSYM, zh = ZSYM;
             if (ASYM) {
-              zl = (float)((cur.zw[ASYM ? gi : 0][ftl * 2] >> (4 * g)) & 15u);
-              zh = (float)((cur.zw[ASYM ? gi : 0][ftl * 2 + 1] >> (4 * g)) & 15u);
+              zl = (float)((lds_u32(sc_a + NG * 64 + gi * 16 + ftl * 8) >> (4 * g)) & 15u);
+              zh = (float)((lds_u32(sc_a + NG * 64 + gi * 16 + ftl * 8 + 4) >> (4 * g)) & 15u);
             }
             const float bl = E::LO_BASE + zl, bh = E::HI_BASE + zh;
             float d[4];
@@ -316,8 +291,7 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
         }
       }
       __syncwarp();
-      if (lane == 0 && iss_u < U) iss_one(ring_a + st * DEC_QUAD_BYTES, bars + 8 * st);
-      if (u + 1 < U) cur = nxt;
+      if (lane == 0 && iss_u < U) iss_one(ring_a + st * DEC_QUAD_BYTES, sring_w + st * SCB, bars + 8 * st);
     }
 
     // park the warp's partial sums of this tile: wpart[(grp, ti, m)][wg][f], f rotated by 8 * (m / 2) so that the four
@@ -433,10 +407,12 @@ __global__ void __launch_bounds__(DEC_MAX_WARPS * 32)
   }
 }
 
-static size_t decode2_smem(int M, int warps, int gw, int qpc, int max_tiles, int ks, int nst) {
+static size_t decode2_smem(const MmArgs& a, int warps, int gw, int qpc, int max_tiles, int ks, int nst) {
+  const int M = a.M, scb = dec_sc_bytes(a.qzeros != nullptr, a.group_size == 64);
   const size_t rows = (size_t)(warps / gw) * max_tiles * M;
   return (size_t)warps * nst * DEC_QUAD_BYTES + (size_t)M * qpc * 128 * 2 + (size_t)qpc * 2 * 8 * 4 +
-         rows * gw * 32 * 4 + (ks > 1 ? rows * 32 * 4 : 0) + (size_t)warps * DEC_STAGES * 8 + 8 + 16;
+         rows * gw * 32 * 4 + (ks > 1 ? rows * 32 * 4 : 0) + (size_t)warps * DEC_STAGES * 8 + 8 + 16 +
+         (size_t)warps * nst * scb;
 }
 
 // Pick (split-K ranks, warps per CTA, warps per group) minimising the critical path in quads per warp.
@@ -462,7 +438,7 @@ bool decode2_config(const MmArgs& a, int NT, DecodePlan& best) {
         if (C < 1) C = 1;
         const int max_tiles = (NT + C * ngroups - 1) / (C * ngroups);  // per group
         DecodePlan p = {C, ks, warps, gw, qpc, max_tiles, 0, 0};
-        if (!fit_ring(p, [&](int nst) { return decode2_smem(a.M, warps, gw, qpc, max_tiles, ks, nst); })) continue;
+        if (!fit_ring(p, [&](int nst) { return decode2_smem(a, warps, gw, qpc, max_tiles, ks, nst); })) continue;
         const int qpw = (qpc + gw - 1) / gw;  // quads per warp per tile
         const double units = (double)max_tiles * qpw;
         // relative cost in units of one quad per warp at 16 warps / SM (heuristic weights); fewer warps hide less
@@ -491,11 +467,16 @@ static int launch_decode2_t(const MmArgs& a, const DecSets& sets, const DecodePl
                        (const T*)a.x, a.M, a.K, decode_gsh(a.group_size), c.qpc, c.max_tiles, c.gw, c.stl, xtma, ar);
 }
 
+int decode2_occupancy(const DecodePlan& c, int* blocks) {  // b2q_decode.cu: decode_occupancy
+  return plan_occupancy(decode2_kernel<__half, false, false, false>, c, blocks);
+}
+
 // Returns -2 when no v2 configuration fits shared memory (the caller falls back to the v1 kernel).
 static int launch_decode2_ar(const MmArgs& a, const DecSets& sets, const DecodeAR& ar) {
   DecodePlan c;
   if (!decode2_config(a, sets.tile_end[sets.nsets - 1], c)) return -2;
   if (ar.world > 1 && c.C * c.ks > DEC_AR_MAXCTA) return -2;
+  if (!sets_aligned(sets, "b2q_decode2")) return -1;
   return dispatch_decode(a, sets, [&](auto inst) { return launch_decode2_t<decltype(inst)>(a, sets, c, ar); });
 }
 

@@ -68,6 +68,7 @@ bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier
 bool decode_supported(const MmArgs& a);
 bool decode_plan(int version, const MmArgs& a, int NT, int* out8);  // launch plan of the decode tier (host only)
+int decode_occupancy(int version, const MmArgs& a, int NT, int* blocks);  // resident CTAs per SM of that plan
 int launch_decode_multi(const MmArgs& a, int nsets, const void* const* packed, const void* const* scales,
                         const int32_t* const* qzeros, const void* const* bias, void* const* out, const int* Ns);
 int launch_gemm(const MmArgs& a);

@@ -194,6 +194,11 @@ void b2q_debug_reload_env(void);
  * tiles (32 features) per group, ring stages, dynamic shared memory bytes}.  ks / warps <= 0 = heuristic. */
 int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, int* out8);
 
+/* Resident CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor on the current device) of the fp16, symmetric,
+ * group-128 instantiation of decode kernel `version`, at the block size and dynamic shared memory of the plan
+ * b2q_debug_decode_plan returns for the same arguments. */
+int b2q_debug_decode_occupancy(int version, int M, int K, int N, int ks, int warps, int* blocks);
+
 /* out[m, k'] = x[m, perm[k']] for 16-bit elements. */
 int b2q_permute_cols(const void* x, const int32_t* perm, void* out, int M, int K, void* stream);
 
