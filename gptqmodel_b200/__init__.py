@@ -5,6 +5,7 @@ Public API:
     B200AwqQuantLinear / awq_gemm_to_gptq   AWQ GEMM-format front-end onto the same kernels
     B200QqqQuantLinear  QQQ (W4A8) checkpoints on the int8 tensor cores
     B200Fp8QuantLinear  FP8 (e4m3fn, W8A16) checkpoints on the 8-bit tiers
+    B200BlockFp8Linear  HF / DeepSeek-native block-FP8 (W8A8) checkpoints on the e4m3 tensor cores
     lib / check       the raw C-ABI (include/b2q.h) through ctypes
 """
 from ._lib import ABI_VERSION, B2QError, LIB_PATH, SYMBOLS, check, lib  # noqa: F401
@@ -13,5 +14,6 @@ from .adapter import Lora  # noqa: F401
 from .awq import B200AwqQuantLinear, awq_gemm_to_gptq  # noqa: F401
 from .qqq import B200QqqQuantLinear  # noqa: F401
 from .fp8 import B200Fp8QuantLinear  # noqa: F401
+from .fp8_block import B200BlockFp8Linear  # noqa: F401
 
-__all__ = ["B200QuantLinear", "B200AwqQuantLinear", "B200QqqQuantLinear", "B200Fp8QuantLinear", "awq_gemm_to_gptq", "Lora", "fuse_siblings", "SiblingGroup", "lib", "check", "B2QError", "LIB_PATH", "SYMBOLS", "ABI_VERSION"]
+__all__ = ["B200QuantLinear", "B200AwqQuantLinear", "B200QqqQuantLinear", "B200Fp8QuantLinear", "B200BlockFp8Linear", "awq_gemm_to_gptq", "Lora", "fuse_siblings", "SiblingGroup", "lib", "check", "B2QError", "LIB_PATH", "SYMBOLS", "ABI_VERSION"]

@@ -52,6 +52,10 @@ SYMBOLS = {
     "b2q_qqq_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     "b2q_fp8_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     "b2q_fp8_dequant": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b2q_fp8blk_workspace_bytes": (_sz, [_i, _i]),
+    "b2q_fp8blk_quantize": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b2q_fp8blk_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8blk_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
 }
 
 

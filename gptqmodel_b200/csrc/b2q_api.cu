@@ -514,6 +514,93 @@ int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, in
                     "b2q_fp8_dequant");
 }
 
+// ---- block-FP8 (HF / DeepSeek-native, W8A8) tier ----
+static size_t fp8blk_codes_bytes(int M, int K) { return ((size_t)M * K + 127) / 128 * 128; }
+
+size_t b2q_fp8blk_workspace_bytes(int M, int K) {
+  if (M <= 8 || K <= 0 || K % 128 != 0) return 0;  // decode quantises inside the GEMM
+  return fp8blk_codes_bytes(M, K) + (size_t)(K / 128) * fp8blk_mp(M) * 4;
+}
+
+static int fp8blk_check_shape(const char* fn, int M, int K, int N, int dtype) {
+  if (M < 0 || K <= 0 || K % 128 != 0 || K > 65536 || N <= 0 || N % 64 != 0) {
+    set_error("%s: shape M=%d K=%d N=%d outside the envelope (M >= 0, K %% 128 == 0, K <= 65536, N %% 64 == 0)", fn, M,
+              K, N);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("%s: dtype=%d not supported (0 fp16, 1 bf16)", fn, dtype);
+    return -2;
+  }
+  return 0;
+}
+
+static int fp8blk_check_layer(const char* fn, const void* weight, const float* s_w, const void* out) {
+  if (weight == nullptr || s_w == nullptr || out == nullptr) {
+    set_error("%s: null pointer argument", fn);
+    return -2;
+  }
+  if (!aligned16(weight) || !aligned16(s_w) || !aligned16(out)) {
+    set_error("%s: weight, s_w and out must be 16-byte aligned", fn);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_fp8blk_quantize(const void* x, void* codes, float* s_x, int M, int K, int dtype, void* stream) {
+  if (int e = fp8blk_check_shape("b2q_fp8blk_quantize", M, K, 64, dtype)) return e;
+  if (M == 0) return 0;
+  if (x == nullptr || codes == nullptr || s_x == nullptr || !aligned16(x) || !aligned16(codes) || !aligned16(s_x)) {
+    set_error("b2q_fp8blk_quantize: x, codes and s_x must be 16-byte aligned device pointers");
+    return -2;
+  }
+  DeviceGuard dg(codes);
+  return check_cuda(launch_fp8blk_quant(x, codes, s_x, M, K, dtype, (cudaStream_t)stream), "b2q_fp8blk_quantize");
+}
+
+int b2q_fp8blk_mm(const void* codes, const float* s_x, const void* weight, const float* s_w, const void* bias,
+                  void* out, int M, int K, int N, int dtype, int ks, void* stream) {
+  if (int e = fp8blk_check_shape("b2q_fp8blk_mm", M, K, N, dtype)) return e;
+  if (int e = fp8blk_check_layer("b2q_fp8blk_mm", weight, s_w, out)) return e;
+  if (ks > 8) {
+    set_error("b2q_fp8blk_mm: ks=%d exceeds the cluster limit 8", ks);
+    return -2;
+  }
+  if (M == 0) return 0;
+  if (codes == nullptr || s_x == nullptr || !aligned16(codes) || !aligned16(s_x)) {
+    set_error("b2q_fp8blk_mm: codes and s_x must be 16-byte aligned device pointers");
+    return -2;
+  }
+  DeviceGuard dg(weight);
+  Fp8BlkArgs a = {nullptr, codes, s_x, weight, s_w, bias, out, M, K, N, dtype, ks, (cudaStream_t)stream};
+  return check_cuda(launch_fp8blk_gemm(a), "b2q_fp8blk_mm");
+}
+
+int b2q_fp8blk_forward(const void* x, const void* weight, const float* s_w, const void* bias, void* out, int M, int K,
+                       int N, int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int e = fp8blk_check_shape("b2q_fp8blk_forward", M, K, N, dtype)) return e;
+  if (int e = fp8blk_check_layer("b2q_fp8blk_forward", weight, s_w, out)) return e;
+  if (M == 0) return 0;
+  const size_t need = b2q_fp8blk_workspace_bytes(M, K);
+  if (x == nullptr || !aligned16(x) || (need > 0 && (workspace == nullptr || !aligned16(workspace) ||
+                                                     workspace_bytes < need))) {
+    set_error("b2q_fp8blk_forward: x and a workspace of b2q_fp8blk_workspace_bytes(M, K) = %zu bytes (16-byte "
+              "aligned) must be given, got %zu", need, workspace_bytes);
+    return -2;
+  }
+  DeviceGuard dg(weight);
+  Fp8BlkArgs a = {x, nullptr, nullptr, weight, s_w, bias, out, M, K, N, dtype, 0, (cudaStream_t)stream};
+  if (M <= 8) return check_cuda(launch_fp8blk_gemm(a), "b2q_fp8blk_forward(fused)");
+  uint8_t* codes = reinterpret_cast<uint8_t*>(workspace);
+  float* s_x = reinterpret_cast<float*>(codes + fp8blk_codes_bytes(M, K));
+  int e = check_cuda(launch_fp8blk_quant(x, codes, s_x, M, K, dtype, (cudaStream_t)stream), "b2q_fp8blk_forward");
+  if (e != 0) return e;
+  a.x = nullptr;
+  a.codes = codes;
+  a.s_x = s_x;
+  return check_cuda(launch_fp8blk_gemm(a), "b2q_fp8blk_forward");
+}
+
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
              const void* bias, void* out, int K, int N, int bits, int group_size, int dtype, int ks, int warps,
              void* stream) {

@@ -1,0 +1,448 @@
+// b2q_fp8blk.cu — block-FP8 (HF / DeepSeek-native, W8A8) tier: e4m3 weights with 128 x 128 block scales times
+// per-token-group e4m3 activations on the e4m3 tensor cores.  include/b2q.h states the arithmetic.  Two kernels:
+//   * fp8blk_quant_kernel: one half-warp per (token, 128-k group): amax, s_x = max(amax, 1e-10) / 448 (IEEE division),
+//     codes = e4m3_rn_satfinite(x / s_x) (IEEE division), written as uint8 [M, K] and fp32 s_x [K/128, Mp].
+//   * fp8blk_gemm_kernel: the structure of qqq_gemm_kernel without dequant warps.  The checkpoint weight [N, K] e4m3 is
+//     already the K-major wgmma A operand: warp 8 loads 128 features x 128 k per k-block straight from it with TMA
+//     (SWIZZLE_128B, rows >= N zero-filled), and the activation codes (B operand, n = NTOK tokens) with their token
+//     scales.  Warpgroup 0 multiplies features 0..63 of the tile, warpgroup 1 features 64..127, each on
+//     m64nNk32.f32.e4m3.e4m3 into a per-block fp32 temporary P that is promoted once per k-block:
+//     acc = fmaf(P, s_x[m] * s_w[tile], acc).  The `ks` CTAs of a cluster split the k-blocks of a tile in contiguous
+//     runs and sum their fp32 partials over distributed shared memory in rank order; token blocks of NTOK rows are
+//     spread over gridDim.z.  No atomics, deterministic for a given launch plan.
+//     Decode (M <= 8, FUSED): there is no quantiser launch.  Warp 8 quantises each k-block of x it hands to the MMA
+//     warps itself, with the same device functions as fp8blk_quant_kernel (1 x 128 groups are local to a k-block), writes
+//     the swizzled B tile and the block's s_x, and fences them to the async proxy.
+#include <cuda.h>
+
+#include <type_traits>
+
+#include "b2q_common.cuh"
+#include "b2q_internal.h"
+#include "b2q_wgmma.cuh"
+
+namespace b2q {
+
+constexpr int F_BF = 128;                 // features per tile (= the checkpoint's scale block rows)
+constexpr int F_BK = 128;                 // k per block (= the scale block columns; one SWIZZLE_128B row of e4m3)
+constexpr int F_MMA_THREADS = 256;        // warps 0..7: two MMA warpgroups
+constexpr int F_THREADS = F_MMA_THREADS + 32;  // + warp 8: producer
+constexpr int F_MAX_KB = 512;             // K <= 65536: the tile's s_w row lives in shared memory
+constexpr int F_QUANT_THREADS = 256;      // quantiser: 16 groups of 128 k per CTA
+
+template <int NTOK>
+struct FblkCfg {
+  static constexpr int ST = NTOK == 128 ? 6 : 8;  // stages
+  static constexpr int W_BYTES = F_BF * F_BK;
+  static constexpr int X_BYTES = NTOK * F_BK;
+  static constexpr int SX_BYTES = NTOK * 4;
+  static constexpr int STAGE_BYTES = (W_BYTES + X_BYTES + SX_BYTES + 1023) / 1024 * 1024;
+  static constexpr int SW_BYTES = F_MAX_KB * 4;
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int SMEM_BYTES = ST * STAGE_BYTES + SW_BYTES + BAR_BYTES + 1024;
+  static constexpr int ACC = NTOK / 2;  // fp32 accumulators per thread of one m64 x NTOK warpgroup tile
+  static_assert(X_BYTES % 1024 == 0, "activation tiles must stay 1024-byte aligned (SWIZZLE_128B atoms)");
+  static_assert(NTOK * F_BF * 4 <= ST * STAGE_BYTES, "the fp32 partial tile reuses the stages");
+  static_assert(2 * ST * 8 <= BAR_BYTES, "mbarrier area");
+  static_assert(SMEM_BYTES <= 227 * 1024, "dynamic shared memory of one CTA");
+};
+
+// ------------------------------------------------------------------------------------------------
+// the quantiser's arithmetic: one device function per step, shared by both kernels so their codes are identical
+// ------------------------------------------------------------------------------------------------
+// A group of 128 k is held by a half-warp, lane j (= lane & 15) owning elements 8 j .. 8 j + 7 in `v`.  All 32 lanes
+// call this (the shuffles span the warp; the halves do not mix): the group's scale max(amax, 1e-10) / 448.
+template <typename T>
+__device__ __forceinline__ float fblk_group_scale(const uint4& v) {
+  const T* h = reinterpret_cast<const T*>(&v);
+  float a = 0.f;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) a = fmaxf(a, fabsf(ET<T>::to_f(h[e])));
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+  return fmaxf(a, 1e-10f) / 448.f;  // IEEE division
+}
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// eight elements -> their eight e4m3 codes, element e in byte e
+template <typename T>
+__device__ __forceinline__ uint2 fblk_code8(const uint4& v, float s) {
+  const T* h = reinterpret_cast<const T*>(&v);
+  float q[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) q[e] = ET<T>::to_f(h[e]) / s;  // IEEE division
+  return make_uint2(e4m3x2(q[0], q[1]) | (e4m3x2(q[2], q[3]) << 16), e4m3x2(q[4], q[5]) | (e4m3x2(q[6], q[7]) << 16));
+}
+
+// one half-warp per (token m, k-block b); lane j of it owns elements 8 j .. 8 j + 7
+template <typename T>
+__global__ void __launch_bounds__(F_QUANT_THREADS)
+    fp8blk_quant_kernel(const T* __restrict__ x, uint8_t* __restrict__ codes, float* __restrict__ s_x, int M, int K,
+                        int Mp) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // x is the previous kernel's output
+  const int KB = K / F_BK;
+  const long long g = ((long long)blockIdx.x * F_QUANT_THREADS + threadIdx.x) >> 4;
+  const int j = threadIdx.x & 15;
+  const bool live = g < (long long)M * KB;  // the whole warp stays for the shuffles
+  const int m = live ? (int)(g / KB) : 0, b = live ? (int)(g % KB) : 0;
+  const size_t off = (size_t)m * K + (size_t)b * F_BK + 8 * j;
+  const uint4 v = live ? *reinterpret_cast<const uint4*>(x + off) : make_uint4(0u, 0u, 0u, 0u);
+  const float s = fblk_group_scale<T>(v);
+  if (!live) return;
+  *reinterpret_cast<uint2*>(codes + off) = fblk_code8<T>(v, s);
+  if (j == 0) s_x[(size_t)b * Mp + m] = s;
+}
+
+// ------------------------------------------------------------------------------------------------
+// GEMM
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+
+// FUSED: 0 = codes and token scales come from fp8blk_quant_kernel (TMA); 1 / 2 = M <= 8, the producer quantises x
+// (fp16 / bf16) itself
+template <int NTOK, int FUSED>
+__global__ void __launch_bounds__(F_THREADS, 1)
+    fp8blk_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                       const __grid_constant__ CUtensorMap tmap_s, const void* __restrict__ x,
+                       const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M,
+                       int K, int N, int kpc, int out_bf16) {
+  using C = FblkCfg<NTOK>;
+  constexpr int ST = C::ST;
+  static_assert(!FUSED || NTOK == 8, "the fused quantiser serves 8-token tiles");
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  // stage s: [W 128 x 128][X NTOK x 128][s_x NTOK]; then the tile's s_w row; then the barriers
+  const uint32_t sSW = smem_base + ST * C::STAGE_BYTES;
+  const uint32_t bar_full = sSW + C::SW_BYTES, bar_empty = bar_full + 8 * ST;
+  const float* sw_s = reinterpret_cast<const float*>(smem + ST * C::STAGE_BYTES);
+  auto sW = [&](int s) { return smem_base + (uint32_t)(s * C::STAGE_BYTES); };
+  auto sX = [&](int s) { return sW(s) + C::W_BYTES; };
+  auto sSX = [&](int s) { return sX(s) + C::X_BYTES; };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nt = blockIdx.x, n0 = nt * F_BF;
+  const int row0 = blockIdx.z * NTOK;
+  const int KB = K / F_BK;
+  const uint32_t nrank = cluster_nctarank(), crank = cluster_ctarank();
+  const int kb0 = min(KB, (int)crank * kpc), kb1 = min(KB, kb0 + kpc);
+  const int nkb = kb1 - kb0;
+
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_w);
+    if (!FUSED) {
+      prefetch_tmap(&tmap_q);
+      prefetch_tmap(&tmap_s);
+    }
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(bar_full + 8 * s, FUSED ? 32 : 1);
+      mbar_init(bar_empty + 8 * s, F_MMA_THREADS / 32);
+    }
+    fence_mbar_init();
+  }
+  // the tile's weight scales (a layer constant: no dependency on the previous kernel)
+  for (int i = threadIdx.x; i < nkb; i += F_THREADS)
+    reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES)[i] = s_w[(size_t)nt * KB + kb0 + i];
+  __syncthreads();
+
+  if (warp == 8) {
+    // ================================ producer ================================
+    auto load_weights = [&](int i, int s) {
+      mbar_expect_tx_only(bar_full + 8 * s, C::W_BYTES);
+      tma_load_2d(sW(s), &tmap_w, bar_full + 8 * s, (kb0 + i) * F_BK, n0);
+    };
+    // the weight stream of the first ST blocks starts at once (under programmatic dependent launch: while the
+    // previous kernel still runs)
+    if (lane == 0)
+      for (int i = 0; i < nkb && i < ST; ++i) load_weights(i, i);
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (FUSED) {
+      using T = typename std::conditional<FUSED == 1, __half, __nv_bfloat16>::type;
+      // the quantiser kernel's mapping: half-warp h of pass p holds token t = 2 p + h, lane j = lane & 15 its elements
+      // 8 j .. 8 j + 7 of the k-block; rows t >= M keep the zero codes and scales written here once
+      constexpr int PD = 4;  // k-blocks of activations in flight ahead of the one being quantised
+      const int h = lane >> 4, j = lane & 15;
+      for (int s = 0; s < ST; ++s) {
+        for (int o = lane; o < C::X_BYTES / 16; o += 32)
+          asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(sX(s) + 16u * o), "r"(0u) : "memory");
+        if (lane < NTOK) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sSX(s) + 4u * lane), "f"(0.f) : "memory");
+      }
+      const T* xr = reinterpret_cast<const T*>(x) + (size_t)kb0 * F_BK + 8 * j;
+      uint4 buf[PD][4];  // [in-flight k-block][pass]
+      auto fetch = [&](int i, uint4(&dst)[4]) {
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const int t = 2 * p + h;
+          dst[p] = (t < M && i < nkb) ? *reinterpret_cast<const uint4*>(xr + (size_t)t * K + (size_t)i * F_BK)
+                                      : make_uint4(0u, 0u, 0u, 0u);
+        }
+      };
+#pragma unroll
+      for (int u = 0; u < PD; ++u) fetch(u, buf[u]);
+      for (int i0 = 0; i0 < nkb; i0 += PD) {
+#pragma unroll
+        for (int u = 0; u < PD; ++u) {
+          const int i = i0 + u;
+          if (i >= nkb) break;
+          const int s = i % ST;
+          uint4 cur[4];
+#pragma unroll
+          for (int p = 0; p < 4; ++p) cur[p] = buf[u][p];
+          fetch(i + PD, buf[u]);
+          if (i >= ST) {
+            mbar_wait(bar_empty + 8 * s, ((i / ST) & 1) ^ 1);
+            if (lane == 0) load_weights(i, s);
+          }
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            if (2 * p >= M) break;  // warp-uniform: both halves take part in the shuffles
+            const int t = 2 * p + h;
+            const float sx = fblk_group_scale<T>(cur[p]);
+            if (t < M) {
+              const uint2 q = fblk_code8<T>(cur[p], sx);
+              const uint32_t addr = sX(s) + (uint32_t)t * 128 + ((((uint32_t)(j >> 1)) ^ (uint32_t)t) << 4) + 8u * (j & 1);
+              asm volatile("st.shared.v2.u32 [%0], {%1,%2};" ::"r"(addr), "r"(q.x), "r"(q.y) : "memory");
+              if (j == 0) asm volatile("st.shared.f32 [%0], %1;" ::"r"(sSX(s) + 4u * t), "f"(sx) : "memory");
+            }
+          }
+          fence_proxy_async_smem();
+          mbar_arrive(bar_full + 8 * s);
+        }
+      }
+    } else if (lane == 0) {
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % ST;
+        if (i >= ST) {
+          mbar_wait(bar_empty + 8 * s, ((i / ST) & 1) ^ 1);
+          load_weights(i, s);
+        }
+        mbar_expect_tx(bar_full + 8 * s, C::X_BYTES + C::SX_BYTES);
+        tma_load_2d(sX(s), &tmap_q, bar_full + 8 * s, (kb0 + i) * F_BK, row0);
+        tma_load_2d(sSX(s), &tmap_s, bar_full + 8 * s, row0, kb0 + i);
+      }
+    }
+  } else {
+    // ================================ MMA warpgroups ================================
+    const int wg = warp >> 2;  // features 64 wg .. 64 wg + 63 of the tile
+    float acc[C::ACC], p[C::ACC];
+#pragma unroll
+    for (int v = 0; v < C::ACC; ++v) acc[v] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % ST;
+      mbar_wait(bar_full + 8 * s, (i / ST) & 1);
+      const uint64_t wdesc = wgmma_desc_k_sw128(sW(s)) + 512 * wg;
+      const uint64_t xdesc = wgmma_desc_k_sw128(sX(s));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < F_BK / 32; ++k) Wgmma8F<NTOK>::mma(p, wdesc + 2 * k, xdesc + 2 * k, k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(p);
+      // promotion: one s_w per tile and k-block, one s_x per token
+      const float sw = sw_s[i];
+      const float* sxs = reinterpret_cast<const float*>(smem + (sSX(s) - smem_base));
+#pragma unroll
+      for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const float sc = sxs[8 * j + 2 * (lane & 3) + c] * sw;
+          acc[4 * j + c] = fmaf(p[4 * j + c], sc, acc[4 * j + c]);
+          acc[4 * j + 2 + c] = fmaf(p[4 * j + 2 + c], sc, acc[4 * j + 2 + c]);
+        }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+    }
+    // both warpgroups are done with the stages before either overwrites them with its partial tile
+    asm volatile("bar.sync 1, %0;" ::"r"(F_MMA_THREADS) : "memory");
+    // this rank's fp32 partial D[feature][token] -> part[token][feature] in its own shared memory
+#pragma unroll
+    for (int v = 0; v < C::ACC; ++v) {
+      const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
+      const int feat = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_base + (uint32_t)(tok * F_BF + feat) * 4), "f"(acc[v])
+                   : "memory");
+    }
+  }
+  __syncwarp();
+  cluster_sync_all();
+  if (warp < F_MMA_THREADS / 32) {
+    // rank z reduces token rows z, z + nrank, ... : the partials of ranks 0, 1, ... added in that order
+    const int nc = n0 + lane * 4;
+    if (nc < N) {
+      for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M;
+           tok += (int)nrank * (F_MMA_THREADS / 32)) {
+        const uint32_t local = smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)lane * 16;
+        float a[4];
+        for (uint32_t r = 0; r < nrank; ++r) {
+          uint32_t ra;
+          float4 v;
+          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
+          asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
+                       : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                       : "r"(ra)
+                       : "memory");
+          if (r == 0) {
+            a[0] = v.x, a[1] = v.y, a[2] = v.z, a[3] = v.w;
+          } else {
+            a[0] += v.x, a[1] += v.y, a[2] += v.z, a[3] += v.w;
+          }
+        }
+        const size_t o = (size_t)(row0 + tok) * N + nc;
+        if (out_bf16) {
+          __nv_bfloat16 y[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            y[e] = __float2bfloat16_rn(a[e]);
+            if (bias != nullptr)
+              y[e] = __float2bfloat16_rn(__bfloat162float(y[e]) +
+                                         __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[nc + e]));
+          }
+          *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = *reinterpret_cast<const uint2*>(y);
+        } else {
+          __half y[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            y[e] = __float2half_rn(a[e]);
+            if (bias != nullptr)
+              y[e] = __float2half_rn(__half2float(y[e]) + __half2float(reinterpret_cast<const __half*>(bias)[nc + e]));
+          }
+          *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out) + o) = *reinterpret_cast<const uint2*>(y);
+        }
+      }
+    }
+  }
+  __syncwarp();
+  cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
+}
+
+// ------------------------------------------------------------------------------------------------
+// host side
+// ------------------------------------------------------------------------------------------------
+typedef CUresult (*FEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// 2-D tensor map (dim0 contiguous, rows `stride` bytes apart) with zero fill past the bounds.  Encoding costs
+// microseconds of host time: cached per thread on every argument.
+static int fblk_tmap(CUtensorMap* map, CUtensorMapDataType dt, const void* p, int dim0, int dim1, size_t stride,
+                     int box0, int box1, CUtensorMapSwizzle sw) {
+  struct Entry {
+    const void* p;
+    int dt, dim0, dim1, box0, box1, sw;
+    size_t stride;
+    CUtensorMap map;
+  };
+  constexpr int NCACHE = 32;
+  static thread_local Entry cache[NCACHE];
+  static thread_local int next = 0, filled = 0;
+  for (int i = 0; i < filled; ++i) {
+    const Entry& c = cache[i];
+    if (c.p == p && c.dt == (int)dt && c.dim0 == dim0 && c.dim1 == dim1 && c.stride == stride && c.box0 == box0 &&
+        c.box1 == box1 && c.sw == (int)sw) {
+      *map = c.map;
+      return 0;
+    }
+  }
+  static FEncodeTiledFn enc = nullptr;
+  if (enc == nullptr) {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      enc = reinterpret_cast<FEncodeTiledFn>(f);
+  }
+  if (enc == nullptr) {
+    set_error("b2q_fp8blk: cuTensorMapEncodeTiled not available from the driver");
+    return -1;
+  }
+  cuuint64_t gdim[2] = {(cuuint64_t)dim0, (cuuint64_t)dim1};
+  cuuint64_t gstride[1] = {(cuuint64_t)stride};
+  cuuint32_t boxd[2] = {(cuuint32_t)box0, (cuuint32_t)box1};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, dt, 2, const_cast<void*>(p), gdim, gstride, boxd, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("b2q_fp8blk: cuTensorMapEncodeTiled failed (%d) for %p [%d, %d] box [%d, %d]", (int)r, p, dim1, dim0,
+              box1, box0);
+    return -1;
+  }
+  Entry& e = cache[next];
+  e = {p, (int)dt, dim0, dim1, box0, box1, (int)sw, stride, *map};
+  next = (next + 1) % NCACHE;
+  if (filled < NCACHE) ++filled;
+  return 0;
+}
+
+int fp8blk_mp(int M) { return (M + 3) / 4 * 4; }
+
+int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream) {
+  const long long threads = (long long)M * (K / F_BK) * 16;
+  const dim3 grid((unsigned)((threads + F_QUANT_THREADS - 1) / F_QUANT_THREADS), 1, 1);
+  if (dtype == 0)
+    return launch_kernel(fp8blk_quant_kernel<__half>, grid, dim3(F_QUANT_THREADS, 1, 1), 0, stream, 0, true,
+                         (const __half*)x, (uint8_t*)codes, s_x, M, K, fp8blk_mp(M));
+  return launch_kernel(fp8blk_quant_kernel<__nv_bfloat16>, grid, dim3(F_QUANT_THREADS, 1, 1), 0, stream, 0, true,
+                       (const __nv_bfloat16*)x, (uint8_t*)codes, s_x, M, K, fp8blk_mp(M));
+}
+
+// tokens per CTA: the narrowest wgmma n that holds M, 128-token blocks beyond
+static int fblk_ntok(int M) { return M <= 8 ? 8 : M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
+
+// split-K ranks: fill the SMs with (tiles x token blocks x ranks) CTAs, at least 2 k-blocks per rank, cluster <= 8
+int fp8blk_ks(int M, int K, int N) {
+  const int KB = K / F_BK, tiles = (N + F_BF - 1) / F_BF, tblocks = (M + fblk_ntok(M) - 1) / fblk_ntok(M);
+  int ks = 1;
+  while (ks < 8 && (long long)tiles * tblocks * ks * 2 <= num_sms() && KB / (ks * 2) >= 2) ks *= 2;
+  while (ks > 1 && (ks - 1) * ((KB + ks - 1) / ks) >= KB) ks >>= 1;  // every rank needs at least one k-block
+  return ks;
+}
+
+template <int NTOK, int FUSED>
+static int launch_fp8blk_gemm_t(const Fp8BlkArgs& a) {
+  using C = FblkCfg<NTOK>;
+  const int KB = a.K / F_BK;
+  CUtensorMap tw, tq, ts;
+  if (fblk_tmap(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, a.N, (size_t)a.K, F_BK, F_BF,
+                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  if (FUSED) {
+    tq = tw;  // unused
+    ts = tw;
+  } else {
+    if (fblk_tmap(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
+                  CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+      return -1;
+    if (fblk_tmap(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, NTOK, 1,
+                  CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
+      return -1;
+  }
+  auto kern = fp8blk_gemm_kernel<NTOK, FUSED>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8blk")) return e;
+  const int tiles = (a.N + F_BF - 1) / F_BF, tblocks = (a.M + NTOK - 1) / NTOK;
+  const int ks = a.ks > 0 ? a.ks : fp8blk_ks(a.M, a.K, a.N);
+  const int kpc = (KB + ks - 1) / ks;
+  return launch_kernel(kern, dim3(tiles, ks, tblocks), dim3(F_THREADS, 1, 1), C::SMEM_BYTES, a.stream, ks, true, tw, tq,
+                       ts, a.x, a.s_w, a.bias, a.out, a.M, a.K, a.N, kpc, a.dtype);
+}
+
+int launch_fp8blk_gemm(const Fp8BlkArgs& a) {
+  if (a.x != nullptr) return a.dtype == 0 ? launch_fp8blk_gemm_t<8, 1>(a) : launch_fp8blk_gemm_t<8, 2>(a);
+  switch (fblk_ntok(a.M)) {
+    case 8: return launch_fp8blk_gemm_t<8, 0>(a);
+    case 16: return launch_fp8blk_gemm_t<16, 0>(a);
+    case 32: return launch_fp8blk_gemm_t<32, 0>(a);
+    case 64: return launch_fp8blk_gemm_t<64, 0>(a);
+    default: return launch_fp8blk_gemm_t<128, 0>(a);
+  }
+}
+
+}  // namespace b2q

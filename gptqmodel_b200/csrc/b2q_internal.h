@@ -63,6 +63,22 @@ struct QqqArgs {
 int launch_qqq_quant(const void* x, void* q, float* s_tok, int M, int K, int dtype, cudaStream_t stream);
 int launch_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int grouped, cudaStream_t stream);
 int launch_qqq_gemm(const QqqArgs& a);
+// block-FP8 (W8A8) tier (b2q_fp8blk.cu)
+struct Fp8BlkArgs {
+  const void* x;          // fused decode (M <= 8): the activations [M, K]; else nullptr
+  const void* codes;      // e4m3 codes [M, K] (x == nullptr)
+  const float* s_x;       // token scales [K/128, fp8blk_mp(M)] (x == nullptr)
+  const void* weight;     // e4m3 [N, K], the checkpoint tensor
+  const float* s_w;       // [ceil(N/128), K/128]
+  const void* bias;       // [N] in the output dtype, or nullptr
+  void* out;              // [M, N]
+  int M, K, N, dtype, ks;  // ks <= 0: heuristic
+  cudaStream_t stream;
+};
+int fp8blk_mp(int M);  // token-scale row length: M rounded up to 4
+int fp8blk_ks(int M, int K, int N);
+int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream);
+int launch_fp8blk_gemm(const Fp8BlkArgs& a);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

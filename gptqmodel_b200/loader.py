@@ -144,7 +144,9 @@ def _parse_fp8(spec: QuantSpec, raw: dict) -> None:
 
     if "activation_scheme" in raw or ("fmt" in raw and "format" not in raw):
         raise NotImplementedError("HF / DeepSeek-native FP8 checkpoints (weight_scale_inv as a multiplier) are not "
-                                  "supported; only the reference's FP8Config (weight = w / weight_scale_inv) is")
+                                  "served here (this entry point reads the reference's FP8Config, weight = w / "
+                                  "weight_scale_inv); load block-FP8 checkpoints with parse_block_fp8_config / "
+                                  "load_block_fp8_linears")
     if raw.get("rotation"):
         raise NotImplementedError("`rotation` is not supported for FP8 checkpoints")
     if int(raw.get("bits", 8)) != 8:
@@ -187,7 +189,7 @@ def fp8_prefixes(names: Iterable[str]) -> list:
     return sorted(n[: -len(sfx)] for n in names if n.endswith(sfx) and n[: -len(sfx)] + ".weight" in names)
 
 
-def read_quant_config(path: str) -> QuantSpec:
+def _read_raw_config(path: str) -> dict:
     for fn in QUANT_CONFIG_FILES:
         p = os.path.join(path, fn)
         if not os.path.exists(p):
@@ -198,8 +200,118 @@ def read_quant_config(path: str) -> QuantSpec:
             raw = raw.get("quantization_config")
             if raw is None:
                 continue
-        return parse_quant_config(raw)
+        return raw
     raise FileNotFoundError(f"no quantisation config ({', '.join(QUANT_CONFIG_FILES)}) under {path}")
+
+
+def read_quant_config(path: str) -> QuantSpec:
+    return parse_quant_config(_read_raw_config(path))
+
+
+@dataclass
+class BlockFp8Spec:
+    """An HF / DeepSeek-native block-FP8 config (transformers' FineGrainedFP8Config)."""
+    weight_block_size: tuple = (128, 128)
+    activation_scheme: str = "dynamic"
+    modules_to_not_convert: Optional[list] = None
+
+
+def parse_block_fp8_config(raw: dict) -> BlockFp8Spec:
+    """`{"quant_method": "fp8", "fmt": "e4m3", "activation_scheme": "dynamic", "weight_block_size": [128, 128]}`:
+    `fmt` may be absent or e4m3, `activation_scheme` absent or dynamic, the block size must be [128, 128].
+    NotImplementedError for what the block-FP8 kernels do not serve (static activations, per-tensor HF FP8, other block
+    sizes, e5m2 / fnuz / e8m0, the reference's own FP8Config), ValueError for malformed entries."""
+    from .fp8 import FP8_FORMAT_ALIASES
+
+    if not isinstance(raw, dict):
+        raise ValueError(f"block FP8: the quantisation config must be a dict, got {type(raw).__name__}")
+    method = raw.get("quant_method", raw.get("method"))
+    if str(method).lower() != "fp8":
+        raise NotImplementedError(f"block FP8: quant_method `{method}` is not fp8")
+    if "format" in raw or "weight_scale_semantics" in raw or "weight_scale_method" in raw:
+        raise NotImplementedError("block FP8: this is the reference's FP8Config (weight = w / weight_scale_inv); load it "
+                                  "with load_quantized_linears")
+    fmt = raw.get("fmt")
+    if fmt is not None:
+        if not isinstance(fmt, str):
+            raise ValueError(f"block FP8: `fmt` must be a string, got {fmt!r}")
+        resolved = FP8_FORMAT_ALIASES.get(fmt.strip().lower())
+        if resolved is None:
+            raise ValueError(f"block FP8: unknown `fmt` `{fmt}`")
+        if resolved != "float8_e4m3fn":
+            raise NotImplementedError(f"block FP8: `fmt` `{fmt}` is not served (e4m3 only)")
+    scheme = raw.get("activation_scheme", "dynamic")
+    if not isinstance(scheme, str):
+        raise ValueError(f"block FP8: `activation_scheme` must be a string, got {scheme!r}")
+    if scheme.strip().lower() == "static":
+        raise NotImplementedError("block FP8: static activation scales (`input_scale`) are not served (dynamic only)")
+    if scheme.strip().lower() != "dynamic":
+        raise ValueError(f"block FP8: unknown `activation_scheme` `{scheme}`")
+    block = raw.get("weight_block_size")
+    if block is None:
+        raise NotImplementedError("block FP8: per-tensor FP8 checkpoints (no `weight_block_size`) are not served")
+    if not isinstance(block, (list, tuple)) or len(block) != 2 or not all(isinstance(b, int) and b > 0 for b in block):
+        raise ValueError(f"block FP8: `weight_block_size` must be two positive integers, got {block!r}")
+    if tuple(block) != (128, 128):
+        raise NotImplementedError(f"block FP8: weight_block_size {list(block)} is not served ([128, 128] only)")
+    skip = raw.get("modules_to_not_convert")
+    if skip is not None and not (isinstance(skip, (list, tuple)) and all(isinstance(s, str) for s in skip)):
+        raise ValueError(f"block FP8: `modules_to_not_convert` must be a list of names, got {skip!r}")
+    return BlockFp8Spec((128, 128), "dynamic", list(skip) if skip is not None else None)
+
+
+@torch.no_grad()
+def load_block_fp8_linears(path: str, device="cuda", dtype: Optional[torch.dtype] = None,
+                           only: Optional[Iterable[str]] = None,
+                           post_init: Optional[bool] = None) -> Dict[str, nn.Module]:
+    """Load every block-FP8 linear of an HF / DeepSeek-native checkpoint into B200BlockFp8Linear modules.
+
+    Modules are the `<prefix>.weight` + `<prefix>.weight_scale_inv` pairs; modules without `weight_scale_inv` (an
+    unquantised lm_head, norms, embeddings) stay dense and are not returned.  Raises ValueError when a scale grid does
+    not fit its weight.
+    only      : optional iterable of module prefixes to load (default: all found)
+    post_init : default True on CUDA devices, False on CPU (tensors only; host tests)
+    """
+    from safetensors import safe_open
+
+    from .fp8_block import B200BlockFp8Linear
+
+    parse_block_fp8_config(_read_raw_config(path))
+    wmap = _weight_map(path)
+    prefixes = list(only) if only is not None else fp8_prefixes(wmap)
+    dev = torch.device(device)
+    do_post = (dev.type == "cuda") if post_init is None else post_init
+    handles: Dict[str, object] = {}
+
+    def tensor(name):
+        fn = wmap.get(name)
+        if fn is None:
+            return None
+        if fn not in handles:
+            handles[fn] = safe_open(fn, framework="pt").__enter__()
+        return handles[fn].get_tensor(name)
+
+    mods: Dict[str, nn.Module] = {}
+    try:
+        for prefix in prefixes:
+            t = {s: tensor(f"{prefix}.{s}") for s in ("weight", "weight_scale_inv", "input_scale", "bias")}
+            if t["weight"] is None or t["weight_scale_inv"] is None:
+                raise KeyError(f"{prefix}: checkpoint misses weight / weight_scale_inv")
+            if t["input_scale"] is not None:
+                raise NotImplementedError(f"{prefix}: static activation scales (`input_scale`) are not served")
+            if t["weight"].dtype != torch.float8_e4m3fn:
+                raise NotImplementedError(f"{prefix}: weight dtype {t['weight'].dtype} is not served "
+                                          "(float8_e4m3fn only)")
+            mods[prefix] = B200BlockFp8Linear.from_checkpoint_tensors(
+                t["weight"], t["weight_scale_inv"], bias=t["bias"], device=dev, dtype=dtype, post_init=do_post,
+                name=prefix)
+    finally:
+        for h in handles.values():
+            close = getattr(h, "__exit__", None)
+            if close is not None:
+                close(None, None, None)
+        handles.clear()
+    return mods
 
 
 def _weight_map(path: str) -> Dict[str, str]:

@@ -246,7 +246,7 @@ class RowParallelLinear(torch.nn.Module):
         if getattr(inner, "online_full_had", False) or getattr(inner, "online_partial_had", False):
             # the online Hadamard transform mixes all K input columns; a row shard holds K / world of them
             raise NotImplementedError("RowParallelLinear: rotated layers (online Hadamard transform) cannot be row-sharded")
-        if getattr(inner, "QUANT_TYPE", None) == "b200_fp8":
+        if getattr(inner, "QUANT_TYPE", None) in ("b200_fp8", "b200_fp8_block"):
             raise NotImplementedError("RowParallelLinear: tensor parallelism of FP8 layers is not supported")
         super().__init__()
         self.inner = inner

@@ -257,6 +257,37 @@ int b2q_fp8_mm(const void* x, const void* packed, const void* scales, const void
 int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
                     void* stream);
 
+/* Block-FP8 (W8A8) layers of HF / DeepSeek-native checkpoints (an addition to ABI v8 that changes no earlier entry
+ * point): `quant_method: fp8`, `fmt: e4m3`, `activation_scheme: dynamic`, `weight_block_size: [128, 128]` (transformers' FineGrainedFP8Config, DeepSeek-V3, the
+ * Qwen3 *-FP8 releases).  Weights e4m3 w [N, K] (the checkpoint tensor, unchanged), s_w = weight_scale_inv fp32
+ * [ceil(N/128), K/128], which MULTIPLIES the weights.  T = fp16 (dtype 0) or bf16 (dtype 1), KB = K / 128.  For every
+ * token row m and k-block b:
+ *   a[m,b]   = max_{k in b} |x[m,k]|                                (exact: x is T, widened to fp32)
+ *   s_x[m,b] = fmaxf(a[m,b], 1e-10f) / 448.f                       (IEEE fp32 division)
+ *   q[m,k]   = e4m3_rn_satfinite(float(x[m,k]) / s_x[m,b])           (IEEE fp32 division)
+ *   P_b[m,n] = sum_{k in b} q[m,k] * w[n,k]                         (e4m3 wgmma, fp32 accumulation)
+ *   acc[m,n] = fmaf(P_b[m,n], s_x[m,b] * s_w[n/128, b], acc[m,n])     for b in increasing order
+ *   y        = T(acc);  y = T(y + bias[n])                          (bias optional, T [N])
+ * The 1e-10 epsilon keeps an all-zero group finite (codes 0).  The fp8 tensor-core accumulator is not an exact fp32 sum,
+ * so P_b is not exact in general; the scales are promoted once per 128-k block.  Split-K: each of the `ks` ranks of a
+ * tile promotes its own contiguous run of k-blocks in order from acc = 0, and the ranks' fp32 partials are added in rank
+ * order.  Results are deterministic for a launch plan; they may differ in the last bits between splits.
+ * Envelope: K % 128 == 0, K <= 65536, N % 64 == 0; x, codes, s_x, weight, s_w, out and workspace 16-byte aligned.
+ * Bad arguments return -2 before any CUDA work. */
+/* Workspace of b2q_fp8blk_forward for M rows: the codes and token scales (0 for M <= 8, which quantise inside the GEMM). */
+size_t b2q_fp8blk_workspace_bytes(int M, int K);
+/* Activation quantiser: x T [M, K] -> codes e4m3 [M, K], s_x fp32 [K/128, Mp] (Mp = M rounded up to 4; s_x[b, m]).
+ * Launched with programmatic dependent launch, so a following b2q_fp8blk_mm starts streaming its weights meanwhile. */
+int b2q_fp8blk_quantize(const void* x, void* codes, float* s_x, int M, int K, int dtype, void* stream);
+/* out T [M, N] from b2q_fp8blk_quantize's codes and scales; ks = split-K ranks (1..8), <= 0: the heuristic. */
+int b2q_fp8blk_mm(const void* codes, const float* s_x, const void* weight, const float* s_w, const void* bias,
+                  void* out, int M, int K, int N, int dtype, int ks, void* stream);
+/* The layer: M <= 8 in ONE launch that quantises the activation blocks it consumes (the codes of b2q_fp8blk_quantize,
+ * the plan of b2q_fp8blk_mm with ks <= 0, so the output is identical to theirs); M > 8 b2q_fp8blk_quantize +
+ * b2q_fp8blk_mm through the workspace.  Dispatches on M inside the library, so a CUDA graph sees the true M. */
+int b2q_fp8blk_forward(const void* x, const void* weight, const float* s_w, const void* bias, void* out, int M, int K,
+                       int N, int dtype, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
