@@ -41,7 +41,8 @@ class SiblingGroup:
     The first member called with a new `x` launches for all members and parks the siblings'
     outputs; each sibling's `forward(x)` then just picks its result up.  Every module keeps the reference's
     per-module `forward(x) -> y` contract (same arithmetic; bit-identical to separate calls whenever the fused launch
-    splits K like the single launches would, see `b2q_debug_decode_plan`); only the launch count changes.
+    splits K like the single launches would, see `b2q_debug_decode_plan`, also when the wide fused launch runs
+    decode2_kernel and a single launch decode_kernel); only the launch count changes.
 
     Contract: parked outputs are keyed on (data_ptr, version, M, dtype) of the activations, are handed out once, and
     are dropped as soon as any member is called with different activations.  The group keeps a strong reference to the

@@ -1,4 +1,6 @@
 """Shared fixtures: synthetic quantised layers built with the oracle's packer (restated pack_original)."""
+import re
+
 import torch
 
 import oracle
@@ -63,6 +65,53 @@ def oracle_forward(layer, x):
     return oracle.forward(xc, layer["qweight"].cpu(), layer["qzeros"].cpu(), layer["scales"].cpu().to(
         torch.float16 if x.dtype == torch.float16 else x.dtype), layer["g_idx"].cpu(), layer["bits"],
         bias=None if layer["bias"] is None else layer["bias"].cpu())
+
+
+_DECODE_KERNEL = re.compile(r"\b(decode2?_kernel)<(__half|__nv_bfloat16), (true|false), (true|false), (true|false)>")
+
+
+def decode_kernels_launched(fn):
+    """Runs fn() under torch.profiler and returns (fn's result, [(kernel, dtype, asym, g64)] of the decode-tier
+    kernels it launched, in launch order): kernel is "decode_kernel" or "decode2_kernel", dtype "__half" or
+    "__nv_bfloat16" — the instantiation that actually ran, whatever the planner predicted."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(3):  # a profiling window this short now and then delivers no kernel record at all: profile again
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            res = fn()
+            torch.cuda.synchronize()
+        evs = sorted((e for e in prof.events() if _DECODE_KERNEL.search(e.name)), key=lambda e: e.time_range.start)
+        if evs:
+            break
+    out = []
+    for e in evs:
+        k, dt, asym, g64, moe = _DECODE_KERNEL.search(e.name).groups()
+        assert moe == "false", e.name
+        out.append((k, dt, asym == "true", g64 == "true"))
+    return res, out
+
+
+def decode_k_split(M, K, N, kernel):
+    """(split-K ranks, warps per tile group, quads per rank) of a decode launch of N features that ran on `kernel`, from
+    that kernel's own planner (b2q_debug_decode_plan, which sizes shared memory for sym g128); None if it has no plan.
+    decode2_kernel picked per launch shape runs one 16-warp group without split-K; B2Q_DECODE_V2=1 lets it choose."""
+    import ctypes
+    import os
+    from gptqmodel_b200 import _lib as g
+    out = (ctypes.c_int * 8)()
+    if kernel == "decode2_kernel":
+        free = os.environ.get("B2Q_DECODE_V2") == "1"
+        rc = g.lib.b2q_debug_decode_plan(2, M, K, N, 0 if free else 1, 0 if free else 16, out)
+    else:
+        rc = g.lib.b2q_debug_decode_plan(1, M, K, N, 0, 0, out)
+    return (out[1], out[3], out[4]) if rc == 0 else None
+
+
+def same_k_split(M, K, single, fused):
+    """True if two decode launches cut K identically; single / fused = (N, kernel that ran).  Both kernels give one
+    warp of a group the same quads and sum the warps' and ranks' fp32 partials in the same order, so two launches with
+    the same (ranks, group width, quads per rank) produce the same bits for a feature, whichever kernel ran."""
+    a, b = decode_k_split(M, K, *single), decode_k_split(M, K, *fused)
+    return a is not None and a == b
 
 
 PARITY_LOG = {}  # test id -> worst err/tol ratio seen by assert_close_rel (dumped by conftest at session end)

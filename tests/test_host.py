@@ -60,6 +60,22 @@ def test_abi_argument_validation_without_gpu():
         assert b"b2q_gemv" in g.lib.b2q_last_error() and b"out of range" in g.lib.b2q_last_error()
         assert g.lib.b2q_decode(one, one, one, None, None, None, one, 1, 128, 64, 4, 128, 0, ks, warps, None) == -2
         assert b"b2q_decode" in g.lib.b2q_last_error() and b"out of range" in g.lib.b2q_last_error()
+    # the decode tier bulk-copies scale / qzeros rows (cp.async.bulk needs 16-byte aligned sources): tensors off by 2
+    # bytes are refused before any CUDA work, on both decode kernels' routes and for every weight set
+    odd = ctypes.c_void_p(16 + 2)
+    for N in (4096, 8192):  # 128 tiles: decode_kernel; 256 tiles (more than SMs): decode2_kernel
+        assert g.lib.b2q_decode(one, one, odd, None, None, None, one, 1, 4096, N, 4, 128, 0, 0, 0, None) != 0
+        assert b"not 16-byte aligned" in g.lib.b2q_last_error()
+        assert g.lib.b2q_decode(one, one, one, odd, None, None, one, 1, 4096, N, 4, 128, 0, 0, 0, None) != 0  # qzeros
+        assert b"not 16-byte aligned" in g.lib.b2q_last_error()
+    vp2 = ctypes.c_void_p * 2
+    for zeros in (vp2(None, None), vp2(16, 16)):
+        assert g.lib.b2q_decode_multi(one, 2, vp2(16, 16), vp2(16, 18), zeros, None, vp2(None, None), vp2(16, 16),
+                                      (ctypes.c_int * 2)(4096, 4096), 1, 4096, 4, 128, 0, None) != 0
+        assert b"set 1 are not 16-byte aligned" in g.lib.b2q_last_error()
+    assert g.lib.b2q_decode_multi(one, 2, vp2(16, 16), vp2(16, 16), vp2(16, 18), None, vp2(None, None), vp2(16, 16),
+                                  (ctypes.c_int * 2)(4096, 4096), 1, 4096, 4, 128, 0, None) != 0
+    assert b"set 1 are not 16-byte aligned" in g.lib.b2q_last_error()
     with pytest.raises(g.B2QError):
         g.check(-2, "x")
 
