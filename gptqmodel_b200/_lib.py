@@ -56,6 +56,9 @@ SYMBOLS = {
     "b2q_fp8blk_quantize": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_fp8blk_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "b2q_fp8blk_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b2q_fp8blk_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8blk_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

@@ -601,6 +601,85 @@ int b2q_fp8blk_forward(const void* x, const void* weight, const float* s_w, cons
   return check_cuda(launch_fp8blk_gemm(a), "b2q_fp8blk_forward");
 }
 
+// ---- block-FP8 MoE experts: the grouped modes of fp8blk_gemm_kernel over the routing tables of b2q_moe_align ----
+static int fp8blk_moe_check(const char* fn, const void* codes, const float* s_x, const void* w, const float* s_w,
+                            const void* out, const int32_t* counts, const int32_t* offsets, int E, int rows, int K, int N,
+                            int dtype, int ks) {
+  if (int e = fp8blk_check_shape(fn, rows, K, N, dtype)) return e;
+  if (int e = fp8blk_check_layer(fn, w, s_w, out)) return e;
+  if (codes == nullptr || s_x == nullptr || counts == nullptr || offsets == nullptr || !aligned16(codes) ||
+      !aligned16(s_x)) {
+    set_error("%s: codes, s_x, counts and offsets must be device pointers, codes and s_x 16-byte aligned", fn);
+    return -2;
+  }
+  if (E < 1 || E > 256 || rows < 1 || ks > 8) {
+    set_error("%s: E=%d (1..256), rows=%d (>= 1), ks=%d (<= 8) outside the envelope", fn, E, rows, ks);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* codes, float* s_x, int T, int top_k, int K,
+                          int dtype, void* stream) {
+  if (T < 1 || top_k < 1) {
+    set_error("b2q_fp8blk_moe_gather: T=%d, top_k=%d must be >= 1", T, top_k);
+    return -2;
+  }
+  if (int e = fp8blk_check_shape("b2q_fp8blk_moe_gather", T * top_k, K, 64, dtype)) return e;
+  if (x == nullptr || sorted_pairs == nullptr || codes == nullptr || s_x == nullptr || !aligned16(x) ||
+      !aligned16(codes) || !aligned16(s_x)) {
+    set_error("b2q_fp8blk_moe_gather: x, sorted_pairs, codes and s_x must be device pointers, x, codes and s_x 16-byte "
+              "aligned");
+    return -2;
+  }
+  DeviceGuard dg(codes);
+  return check_cuda(launch_fp8blk_moe_gather(x, sorted_pairs, codes, s_x, T * top_k, top_k, K, dtype,
+                                             (cudaStream_t)stream),
+                    "b2q_fp8blk_moe_gather");
+}
+
+int b2q_fp8blk_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                           const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                           int active, int K, int N, int dtype, int ks, void* stream) {
+  if (int e = fp8blk_moe_check("b2q_fp8blk_moe_gate_up", codes, s_x, w1, s_w1, h, counts, offsets, E, rows, K, N, dtype,
+                               ks))
+    return e;
+  if (int e = fp8blk_check_layer("b2q_fp8blk_moe_gate_up", w3, s_w3, h)) return e;
+  DeviceGuard dg(w1);
+  Fp8BlkArgs a = {nullptr, codes, s_x, w1, s_w1, nullptr, h, rows, K, N, dtype, ks, (cudaStream_t)stream};
+  Fp8BlkMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.w3 = w3;
+  g.s_w3 = s_w3;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_fp8blk_moe(1, a, g), "b2q_fp8blk_moe_gate_up");
+}
+
+int b2q_fp8blk_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                        const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                        int E, int rows, int active, int K, int N, int dtype, int ks, void* stream) {
+  if (int e = fp8blk_moe_check("b2q_fp8blk_moe_down", codes_h, s_h, w2, s_w2, ypair, counts, offsets, E, rows, K, N,
+                               dtype, ks))
+    return e;
+  if (sorted_pairs == nullptr || pair_weights == nullptr) {
+    set_error("b2q_fp8blk_moe_down: sorted_pairs and pair_weights must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(w2);
+  Fp8BlkArgs a = {nullptr, codes_h, s_h, w2, s_w2, nullptr, ypair, rows, K, N, dtype, ks, (cudaStream_t)stream};
+  Fp8BlkMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.sorted_pairs = sorted_pairs;
+  g.pair_weights = pair_weights;
+  g.ypair = ypair;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_fp8blk_moe(2, a, g), "b2q_fp8blk_moe_down");
+}
+
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
              const void* bias, void* out, int K, int N, int bits, int group_size, int dtype, int ks, int warps,
              void* stream) {

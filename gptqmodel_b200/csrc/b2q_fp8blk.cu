@@ -1,5 +1,5 @@
 // b2q_fp8blk.cu — block-FP8 (HF / DeepSeek-native, W8A8) tier: e4m3 weights with 128 x 128 block scales times
-// per-token-group e4m3 activations on the e4m3 tensor cores.  include/b2q.h states the arithmetic.  Two kernels:
+// per-token-group e4m3 activations on the e4m3 tensor cores.  include/b2q.h states the arithmetic.  Kernels:
 //   * fp8blk_quant_kernel: one half-warp per (token, 128-k group): amax, s_x = max(amax, 1e-10) / 448 (IEEE division),
 //     codes = e4m3_rn_satfinite(x / s_x) (IEEE division), written as uint8 [M, K] and fp32 s_x [K/128, Mp].
 //   * fp8blk_gemm_kernel: the structure of qqq_gemm_kernel without dequant warps.  The checkpoint weight [N, K] e4m3 is
@@ -13,6 +13,12 @@
 //     Decode (M <= 8, FUSED): there is no quantiser launch.  Warp 8 quantises each k-block of x it hands to the MMA
 //     warps itself, with the same device functions as fp8blk_quant_kernel (1 x 128 groups are local to a k-block), writes
 //     the swizzled B tile and the block's s_x, and fences them to the async proxy.
+//   * fp8blk_moe_gemm_kernel: grouped modes of the same GEMM body for MoE experts (MODE 1 / 2): z0 + blockIdx.z =
+//     (expert, token block) over the expert-sorted rows that b2q_moe_align ordered; the weights are the stacked
+//     checkpoint tensors [E*N, K] and [E, ceil(N/128), K/128].  MODE 1
+//     pairs 64 gate features (w1, warpgroup 0) with the same 64 up features (w3, warpgroup 1) in one 128-row tile and
+//     stores h = T(T(silu(T(g))) * T(u)); MODE 2 (down) stores w[pair] * T(acc) in fp32 to the pair's row of ypair.
+//   * fp8blk_moe_gather_kernel: the quantiser over the sorted rows, row i reading token sorted_pairs[i] / top_k.
 #include <cuda.h>
 
 #include <type_traits>
@@ -30,14 +36,16 @@ constexpr int F_THREADS = F_MMA_THREADS + 32;  // + warp 8: producer
 constexpr int F_MAX_KB = 512;             // K <= 65536: the tile's s_w row lives in shared memory
 constexpr int F_QUANT_THREADS = 256;      // quantiser: 16 groups of 128 k per CTA
 
-template <int NTOK>
+template <int NTOK, int MODE = 0>
 struct FblkCfg {
   static constexpr int ST = NTOK == 128 ? 6 : 8;  // stages
   static constexpr int W_BYTES = F_BF * F_BK;
   static constexpr int X_BYTES = NTOK * F_BK;
-  static constexpr int SX_BYTES = NTOK * 4;
+  // grouped modes: a block's first row is any row, so its token scales are loaded from the 16-byte aligned row below it
+  // (4 more scales) — the innermost TMA coordinate stays 16-byte aligned
+  static constexpr int SX_BYTES = (NTOK + (MODE != 0 ? 4 : 0)) * 4;
   static constexpr int STAGE_BYTES = (W_BYTES + X_BYTES + SX_BYTES + 1023) / 1024 * 1024;
-  static constexpr int SW_BYTES = F_MAX_KB * 4;
+  static constexpr int SW_BYTES = (MODE == 1 ? 2 : 1) * F_MAX_KB * 4;  // MODE 1: the gate row, then the up row
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = ST * STAGE_BYTES + SW_BYTES + BAR_BYTES + 1024;
   static constexpr int ACC = NTOK / 2;  // fp32 accumulators per thread of one m64 x NTOK warpgroup tile
@@ -97,6 +105,28 @@ __global__ void __launch_bounds__(F_QUANT_THREADS)
   if (j == 0) s_x[(size_t)b * Mp + m] = s;
 }
 
+// the quantiser over the expert-sorted rows of a MoE block: row i is token sorted_pairs[i] / top_k of x [T, K], so its
+// codes and scale are those fp8blk_quant_kernel gives that token
+template <typename T>
+__global__ void __launch_bounds__(F_QUANT_THREADS)
+    fp8blk_moe_gather_kernel(const T* __restrict__ x, const int32_t* __restrict__ sorted_pairs,
+                             uint8_t* __restrict__ codes, float* __restrict__ s_x, int rows, int top_k, int K, int Mp) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // sorted_pairs (and x) are the previous kernels' output
+  const int KB = K / F_BK;
+  const long long g = ((long long)blockIdx.x * F_QUANT_THREADS + threadIdx.x) >> 4;
+  const int j = threadIdx.x & 15;
+  const bool live = g < (long long)rows * KB;  // the whole warp stays for the shuffles
+  const int i = live ? (int)(g / KB) : 0, b = live ? (int)(g % KB) : 0;
+  const int tok = live ? sorted_pairs[i] / top_k : 0;
+  const uint4 v = live ? *reinterpret_cast<const uint4*>(x + (size_t)tok * K + (size_t)b * F_BK + 8 * j)
+                       : make_uint4(0u, 0u, 0u, 0u);
+  const float s = fblk_group_scale<T>(v);
+  if (!live) return;
+  *reinterpret_cast<uint2*>(codes + (size_t)i * K + (size_t)b * F_BK + 8 * j) = fblk_code8<T>(v, s);
+  if (j == 0) s_x[(size_t)b * Mp + i] = s;
+}
+
 // ------------------------------------------------------------------------------------------------
 // GEMM
 // ------------------------------------------------------------------------------------------------
@@ -104,17 +134,47 @@ __device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes
   asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 
+// MODE 1: h[i, c] = T(T(silu(g)) * u) with g, u the T-rounded products of w1 and w3
+template <typename T>
+__device__ __forceinline__ uint32_t fblk_silu_mul2(float g0, float g1, float u0, float u1) {
+  using E = ET<T>;
+  const float g[2] = {g0, g1}, u[2] = {u0, u1};
+  float h[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float gq = E::to_f(E::from_f(g[i])), uq = E::to_f(E::from_f(u[i]));
+    const float aq = E::to_f(E::from_f(gq / (1.f + __expf(-gq))));
+    h[i] = aq * uq;
+  }
+  return E::pack2(h[0], h[1]);
+}
+
+// grouped launches (MODE 1 / 2) over the experts of a MoE block
+struct FblkMoeArgs {
+  CUtensorMap tmap_w3;           // MODE 1: the w3 stack [E*N, K], 64-row boxes (tmap_w: the w1 stack, the same boxes)
+  const int32_t* counts;         // [E] rows of expert e
+  const int32_t* offsets;        // [E] first sorted row of expert e
+  const int32_t* sorted_pairs;   // [rows] pair index (token * top_k + j) of sorted row i   (MODE 2)
+  const float* pair_weights;     // [rows] routing weight by pair index                     (MODE 2)
+  const float* s_w3;             // [E, ceil(N/128), K/128] scales of w3                     (MODE 1)
+  float* ypair;                  // [rows, N] fp32, row = pair index                          (MODE 2)
+  int tblocks;                   // token blocks of NTOK rows per expert
+  int z0;                        // (expert, token block) of blockIdx.z == 0 (grids over 65535 blocks are split)
+};
+
+// the GEMM of fp8blk_gemm_kernel (MODE 0) and fp8blk_moe_gemm_kernel (MODE 1 / 2, G their grouped arguments).
 // FUSED: 0 = codes and token scales come from fp8blk_quant_kernel (TMA); 1 / 2 = M <= 8, the producer quantises x
-// (fp16 / bf16) itself
-template <int NTOK, int FUSED>
-__global__ void __launch_bounds__(F_THREADS, 1)
-    fp8blk_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
-                       const __grid_constant__ CUtensorMap tmap_s, const void* __restrict__ x,
-                       const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M,
-                       int K, int N, int kpc, int out_bf16) {
-  using C = FblkCfg<NTOK>;
+// (fp16 / bf16) itself.  MODE: 0 = one layer, 1 = grouped gate|up, 2 = grouped down (FUSED == 0)
+template <int NTOK, int FUSED, int MODE>
+__device__ __forceinline__ void fp8blk_gemm_body(const CUtensorMap& tmap_w, const CUtensorMap& tmap_q,
+                                                 const CUtensorMap& tmap_s, const void* __restrict__ x,
+                                                 const float* __restrict__ s_w, const void* __restrict__ bias,
+                                                 void* __restrict__ out, int M, int K, int N, int kpc, int out_bf16,
+                                                 const FblkMoeArgs* G) {
+  using C = FblkCfg<NTOK, MODE>;
   constexpr int ST = C::ST;
   static_assert(!FUSED || NTOK == 8, "the fused quantiser serves 8-token tiles");
+  static_assert(MODE == 0 || !FUSED, "the grouped modes read quantised codes");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -127,8 +187,20 @@ __global__ void __launch_bounds__(F_THREADS, 1)
   auto sSX = [&](int s) { return sX(s) + C::X_BYTES; };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nt = blockIdx.x, n0 = nt * F_BF;
-  const int row0 = blockIdx.z * NTOK;
+  const int nt = blockIdx.x, n0 = nt * (MODE == 1 ? F_BF / 2 : F_BF);  // MODE 1: 64 gate + 64 up features
+  int row0 = blockIdx.z * NTOK;
+  int e = 0;  // expert (grouped modes)
+  if (MODE != 0) {
+    // the routing tables are the output of the preceding kernels: nothing may be read before they have finished
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int z = G->z0 + (int)blockIdx.z;
+    e = z / G->tblocks;
+    const int tb = z - e * G->tblocks, cnt = G->counts[e];
+    if (tb * NTOK >= cnt) return;  // the same decision in every CTA of the cluster (they differ in blockIdx.y only)
+    row0 = G->offsets[e] + tb * NTOK;
+    M = row0 + min(NTOK, cnt - tb * NTOK);  // the stores stop at the expert's last row
+  }
+  const int wrow = MODE == 0 ? n0 : e * N + n0;  // first row of the tile in the (stacked) weight tensor
   const int KB = K / F_BK;
   const uint32_t nrank = cluster_nctarank(), crank = cluster_ctarank();
   const int kb0 = min(KB, (int)crank * kpc), kb1 = min(KB, kb0 + kpc);
@@ -138,6 +210,7 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_w);
+    if (MODE == 1) prefetch_tmap(&G->tmap_w3);
     if (!FUSED) {
       prefetch_tmap(&tmap_q);
       prefetch_tmap(&tmap_s);
@@ -149,15 +222,26 @@ __global__ void __launch_bounds__(F_THREADS, 1)
     fence_mbar_init();
   }
   // the tile's weight scales (a layer constant: no dependency on the previous kernel)
-  for (int i = threadIdx.x; i < nkb; i += F_THREADS)
-    reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES)[i] = s_w[(size_t)nt * KB + kb0 + i];
+  if (MODE == 0) {
+    for (int i = threadIdx.x; i < nkb; i += F_THREADS)
+      reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES)[i] = s_w[(size_t)nt * KB + kb0 + i];
+  } else {
+    // the scale row of the tile's features in expert e's [ceil(N/128), K/128] grid (MODE 1: of the gate and the up set)
+    const size_t sr = ((size_t)e * ((N + F_BF - 1) / F_BF) + n0 / F_BF) * KB + kb0;
+    for (int i = threadIdx.x; i < nkb; i += F_THREADS) {
+      reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES)[i] = s_w[sr + i];
+      if (MODE == 1) reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES)[F_MAX_KB + i] = G->s_w3[sr + i];
+    }
+  }
   __syncthreads();
 
   if (warp == 8) {
     // ================================ producer ================================
     auto load_weights = [&](int i, int s) {
       mbar_expect_tx_only(bar_full + 8 * s, C::W_BYTES);
-      tma_load_2d(sW(s), &tmap_w, bar_full + 8 * s, (kb0 + i) * F_BK, n0);
+      tma_load_2d(sW(s), &tmap_w, bar_full + 8 * s, (kb0 + i) * F_BK, wrow);
+      // MODE 1: the up features' 64-row box fills the second m64 half of the tile
+      if (MODE == 1) tma_load_2d(sW(s) + C::W_BYTES / 2, &G->tmap_w3, bar_full + 8 * s, (kb0 + i) * F_BK, wrow);
     };
     // the weight stream of the first ST blocks starts at once (under programmatic dependent launch: while the
     // previous kernel still runs)
@@ -226,7 +310,7 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         }
         mbar_expect_tx(bar_full + 8 * s, C::X_BYTES + C::SX_BYTES);
         tma_load_2d(sX(s), &tmap_q, bar_full + 8 * s, (kb0 + i) * F_BK, row0);
-        tma_load_2d(sSX(s), &tmap_s, bar_full + 8 * s, row0, kb0 + i);
+        tma_load_2d(sSX(s), &tmap_s, bar_full + 8 * s, MODE == 0 ? row0 : row0 & ~3, kb0 + i);
       }
     }
   } else {
@@ -247,8 +331,8 @@ __global__ void __launch_bounds__(F_THREADS, 1)
       wgmma_wait<0>();
       wgmma_fence_regs(p);
       // promotion: one s_w per tile and k-block, one s_x per token
-      const float sw = sw_s[i];
-      const float* sxs = reinterpret_cast<const float*>(smem + (sSX(s) - smem_base));
+      const float sw = sw_s[(MODE == 1 ? wg * F_MAX_KB : 0) + i];
+      const float* sxs = reinterpret_cast<const float*>(smem + (sSX(s) - smem_base)) + (MODE == 0 ? 0 : row0 & 3);
 #pragma unroll
       for (int j = 0; j < NTOK / 8; ++j)
 #pragma unroll
@@ -273,7 +357,30 @@ __global__ void __launch_bounds__(F_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();
-  if (warp < F_MMA_THREADS / 32) {
+  if (MODE == 1 && warp < F_MMA_THREADS / 32) {
+    // lane l: gate features 2l, 2l + 1 of the tile (columns n0 + 2l, n0 + 2l + 1 of h) and their up features at + 64;
+    // the ranks' partials added in rank order as below
+    for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M; tok += (int)nrank * (F_MMA_THREADS / 32)) {
+      const uint32_t local = smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)lane * 8;
+      float g[2], u[2];
+      for (uint32_t r = 0; r < nrank; ++r) {
+        uint32_t ra;
+        float2 vg, vu;
+        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
+        asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];" : "=f"(vg.x), "=f"(vg.y) : "r"(ra) : "memory");
+        asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];" : "=f"(vu.x), "=f"(vu.y) : "r"(ra + (F_BF / 2) * 4)
+                     : "memory");
+        if (r == 0) {
+          g[0] = vg.x, g[1] = vg.y, u[0] = vu.x, u[1] = vu.y;
+        } else {
+          g[0] += vg.x, g[1] += vg.y, u[0] += vu.x, u[1] += vu.y;
+        }
+      }
+      const uint32_t hv = out_bf16 ? fblk_silu_mul2<__nv_bfloat16>(g[0], g[1], u[0], u[1])
+                                   : fblk_silu_mul2<__half>(g[0], g[1], u[0], u[1]);
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(out) + (size_t)(row0 + tok) * N + n0 + 2 * lane) = hv;
+    }
+  } else if (MODE != 1 && warp < F_MMA_THREADS / 32) {
     // rank z reduces token rows z, z + nrank, ... : the partials of ranks 0, 1, ... added in that order
     const int nc = n0 + lane * 4;
     if (nc < N) {
@@ -296,7 +403,21 @@ __global__ void __launch_bounds__(F_THREADS, 1)
           }
         }
         const size_t o = (size_t)(row0 + tok) * N + nc;
-        if (out_bf16) {
+        if (MODE == 2) {
+          // T(h W2) like the module, times the routing weight, in fp32 in the pair's row: moe_combine_kernel sums the
+          // top_k rows of a token and rounds once
+          const int pair = G->sorted_pairs[row0 + tok];
+          const float w = G->pair_weights[pair];
+          float4 y;
+          if (out_bf16) {
+            y = make_float4(w * __bfloat162float(__float2bfloat16_rn(a[0])), w * __bfloat162float(__float2bfloat16_rn(a[1])),
+                            w * __bfloat162float(__float2bfloat16_rn(a[2])), w * __bfloat162float(__float2bfloat16_rn(a[3])));
+          } else {
+            y = make_float4(w * __half2float(__float2half_rn(a[0])), w * __half2float(__float2half_rn(a[1])),
+                            w * __half2float(__float2half_rn(a[2])), w * __half2float(__float2half_rn(a[3])));
+          }
+          *reinterpret_cast<float4*>(G->ypair + (size_t)pair * N + nc) = y;
+        } else if (out_bf16) {
           __nv_bfloat16 y[4];
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
@@ -321,6 +442,25 @@ __global__ void __launch_bounds__(F_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
+}
+
+template <int NTOK, int FUSED>
+__global__ void __launch_bounds__(F_THREADS, 1)
+    fp8blk_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                       const __grid_constant__ CUtensorMap tmap_s, const void* __restrict__ x,
+                       const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M,
+                       int K, int N, int kpc, int out_bf16) {
+  fp8blk_gemm_body<NTOK, FUSED, 0>(tmap_w, tmap_q, tmap_s, x, s_w, bias, out, M, K, N, kpc, out_bf16, nullptr);
+}
+
+// grouped launches over the experts of a MoE block: M = rows, N / K of one expert, out = h (MODE 1)
+template <int NTOK, int MODE>
+__global__ void __launch_bounds__(F_THREADS, 1)
+    fp8blk_moe_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                           const __grid_constant__ CUtensorMap tmap_s, const float* __restrict__ s_w,
+                           void* __restrict__ out, int M, int K, int N, int kpc, int out_bf16,
+                           const __grid_constant__ FblkMoeArgs G) {
+  fp8blk_gemm_body<NTOK, 0, MODE>(tmap_w, tmap_q, tmap_s, nullptr, s_w, nullptr, out, M, K, N, kpc, out_bf16, &G);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -443,6 +583,89 @@ int launch_fp8blk_gemm(const Fp8BlkArgs& a) {
     case 64: return launch_fp8blk_gemm_t<64, 0>(a);
     default: return launch_fp8blk_gemm_t<128, 0>(a);
   }
+}
+
+int launch_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* codes, float* s_x, int rows, int top_k,
+                             int K, int dtype, cudaStream_t stream) {
+  const long long threads = (long long)rows * (K / F_BK) * 16;
+  const dim3 grid((unsigned)((threads + F_QUANT_THREADS - 1) / F_QUANT_THREADS), 1, 1);
+  if (dtype == 0)
+    return launch_kernel(fp8blk_moe_gather_kernel<__half>, grid, dim3(F_QUANT_THREADS, 1, 1), 0, stream, 0, true,
+                         (const __half*)x, sorted_pairs, (uint8_t*)codes, s_x, rows, top_k, K, fp8blk_mp(rows));
+  return launch_kernel(fp8blk_moe_gather_kernel<__nv_bfloat16>, grid, dim3(F_QUANT_THREADS, 1, 1), 0, stream, 0, true,
+                       (const __nv_bfloat16*)x, sorted_pairs, (uint8_t*)codes, s_x, rows, top_k, K, fp8blk_mp(rows));
+}
+
+// split-K ranks of a grouped launch: fp8blk_ks with `active` experts' token blocks in place of the layer's
+int fp8blk_moe_ks(int rows, int K, int N, int mode, int active) {
+  const int KB = K / F_BK, tiles = (N + (mode == 1 ? F_BF / 2 : F_BF) - 1) / (mode == 1 ? F_BF / 2 : F_BF);
+  const int per = (rows + fblk_ntok(rows) - 1) / fblk_ntok(rows);  // token blocks of all rows
+  const long long blocks = (long long)tiles * (per > active ? per : active);
+  int ks = 1;
+  while (ks < 8 && blocks * ks * 2 <= num_sms() && KB / (ks * 2) >= 2) ks *= 2;
+  while (ks > 1 && (ks - 1) * ((KB + ks - 1) / ks) >= KB) ks >>= 1;  // every rank needs at least one k-block
+  return ks;
+}
+
+template <int NTOK, int MODE>
+static int launch_fp8blk_moe_t(const Fp8BlkArgs& a, const Fp8BlkMoe& g, int ks) {
+  using C = FblkCfg<NTOK, MODE>;
+  const int KB = a.K / F_BK;
+  const int wbox = MODE == 1 ? F_BF / 2 : F_BF;
+  FblkMoeArgs G = {};
+  CUtensorMap tw, tq, ts;
+  if (fblk_tmap(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
+                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  if (MODE == 1 && fblk_tmap(&G.tmap_w3, CU_TENSOR_MAP_DATA_TYPE_UINT8, g.w3, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
+                             CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  if (fblk_tmap(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
+                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  if (fblk_tmap(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, C::SX_BYTES / 4, 1,
+                CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
+    return -1;
+  G.counts = g.counts;
+  G.offsets = g.offsets;
+  G.sorted_pairs = g.sorted_pairs;
+  G.pair_weights = g.pair_weights;
+  G.s_w3 = g.s_w3;
+  G.ypair = g.ypair;
+  G.tblocks = (a.M + NTOK - 1) / NTOK;
+  auto kern = fp8blk_moe_gemm_kernel<NTOK, MODE>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8blk_moe")) return e;
+  const int tiles = (a.N + wbox - 1) / wbox;
+  const int kpc = (KB + ks - 1) / ks;
+  // gridDim.z is at most 65535: a larger (expert, token block) grid is issued as consecutive launches over ranges of z.
+  // They stay ordered under programmatic dependent launch: every CTA executes griddepcontrol.wait before it can exit.
+  constexpr int MAX_Z = 65535;
+  const long long total_z = (long long)g.E * G.tblocks;
+  for (long long z0 = 0; z0 < total_z; z0 += MAX_Z) {
+    G.z0 = (int)z0;
+    const int grid_z = (int)(total_z - z0 < MAX_Z ? total_z - z0 : MAX_Z);
+    const int e = launch_kernel(kern, dim3(tiles, ks, grid_z), dim3(F_THREADS, 1, 1), C::SMEM_BYTES, a.stream, ks, true,
+                                tw, tq, ts, a.s_w, a.out, a.M, a.K, a.N, kpc, a.dtype, G);
+    if (e != 0) return e;
+  }
+  return 0;
+}
+
+int launch_fp8blk_moe(int mode, const Fp8BlkArgs& a, const Fp8BlkMoe& g) {
+  // a pinned ks is taken as given, like b2q_fp8blk_mm's, so both run the same split
+  const int ks = a.ks > 0 ? a.ks : fp8blk_moe_ks(a.M, a.K, a.N, mode, g.active > 0 ? g.active : 1);
+#define B2Q_FBM(MODE)                                                    \
+  switch (fblk_ntok(a.M)) {                                               \
+    case 8: return launch_fp8blk_moe_t<8, MODE>(a, g, ks);                \
+    case 16: return launch_fp8blk_moe_t<16, MODE>(a, g, ks);              \
+    case 32: return launch_fp8blk_moe_t<32, MODE>(a, g, ks);              \
+    case 64: return launch_fp8blk_moe_t<64, MODE>(a, g, ks);              \
+    default: return launch_fp8blk_moe_t<128, MODE>(a, g, ks);             \
+  }
+  if (mode == 1) B2Q_FBM(1)
+  B2Q_FBM(2)
+#undef B2Q_FBM
 }
 
 }  // namespace b2q

@@ -79,6 +79,22 @@ int fp8blk_mp(int M);  // token-scale row length: M rounded up to 4
 int fp8blk_ks(int M, int K, int N);
 int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream);
 int launch_fp8blk_gemm(const Fp8BlkArgs& a);
+// grouped (MoE) launches of the block-FP8 GEMM: a = {codes / s_x = the expert-sorted rows [M = rows, K], weight / s_w =
+// the stacked w1 (mode 1) or w2 (mode 2) [E*N, K] / [E, ceil(N/128), K/128], out = h [rows, N] (mode 1), N / K of ONE
+// expert, ks <= 0: heuristic}
+struct Fp8BlkMoe {
+  const int32_t* counts;        // [E]
+  const int32_t* offsets;       // [E]
+  const int32_t* sorted_pairs;  // [rows]     (mode 2)
+  const float* pair_weights;    // [rows]     (mode 2)
+  const void* w3;               // mode 1: the up stack, shaped like the gate stack
+  const float* s_w3;
+  float* ypair;                 // mode 2: [rows, N] fp32
+  int E, active;                // experts, experts expected to be active (grid sizing only)
+};
+int launch_fp8blk_moe(int mode, const Fp8BlkArgs& a, const Fp8BlkMoe& g);
+int launch_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* codes, float* s_x, int rows, int top_k,
+                             int K, int dtype, cudaStream_t stream);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

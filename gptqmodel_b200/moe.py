@@ -18,6 +18,11 @@ per-expert loop, arranged for the B200 kernels and for tensor parallelism:
     width for w1 / w3 and one for w2.  Act-order experts were prepacked with their rows in group order: the gather reads
     each expert's activations in that expert's column order (`b2q_moe_gather_perm`), and a w2 with act-order gets h
     permuted the same way before the down launch (six launches);
+  * BLOCK-FP8 experts (every w1 / w3 / w2 a post_init'ed B200BlockFp8Linear, HF / DeepSeek-native checkpoints): the same
+    routing with no host synchronisation, six launches on the e4m3 tensor cores — align, gather-and-quantise, ONE grouped
+    gate|up launch, the quantiser on h, ONE grouped down launch, combine (grouped modes of b2q_fp8blk.cu; include/b2q.h
+    states the rounding points, those of transformers' per-expert FP8Linear loop).  The checkpoint tensors are stacked
+    once and the modules keep views into the stack;
   * LOOP path (fallback: dense stand-ins in CPU tests, mixed experts, regrouped act-order shards): tokens are sorted by
     expert once, every expert sees one contiguous block of its routed tokens; one host sync per block for the per-expert
     counts, like the reference's loop;
@@ -70,7 +75,8 @@ class MoEExperts(torch.nn.Module):
                 raise ValueError("MoEExperts(grouped=True): experts must be post_init'ed B200 QuantLinears of one shape / "
                                  "group size, with one kernel bit width (4 or 8) for w1 / w3 and one for w2, the same "
                                  "act-order permutation in w1 and w3 of every expert, and no regrouped g_idx, bias or "
-                                 "adapters")
+                                 "adapters; or post_init'ed B200BlockFp8Linears only, one shape per role on one device, "
+                                 "an intermediate size that is a multiple of 128, and no bias or adapters")
         if fuse and self._stack is None:
             from .qlinear import B200KernelMixin, fuse_siblings
 
@@ -80,8 +86,11 @@ class MoEExperts(torch.nn.Module):
 
     def _build_stack(self):
         """Stack the experts' prepacked tensors for the grouped kernels; None if the experts do not qualify."""
+        from .fp8_block import B200BlockFp8Linear
         from .qlinear import B200KernelMixin
 
+        if all(isinstance(m, B200BlockFp8Linear) for mods in (self.w1, self.w3, self.w2) for m in mods):
+            return self._build_fp8blk_stack()
         sets = []
         for mods in (self.w1, self.w3, self.w2):
             m0 = mods[0]
@@ -129,6 +138,79 @@ class MoEExperts(torch.nn.Module):
             out[name] = dict(packed=packed, scales={scales.dtype: scales}, zeros=zeros, K=mods[0].in_features,
                              N=mods[0].out_features, group=mods[0].group_size, bits=mods[0].kbits, perm=perm)
         return out
+
+    def _build_fp8blk_stack(self):
+        """Stack the block-FP8 experts' checkpoint tensors (weight [E, N, K] e4m3, weight_scale_inv [E, ceil(N/128),
+        K/128]) for the grouped kernels; None if the experts do not qualify."""
+        w1, w3, w2 = list(self.w1), list(self.w3), list(self.w2)
+        for mods in (w1, w3, w2):
+            m0 = mods[0]
+            for m in mods:
+                if not m._ready or m.bias is not None or m.adapter:
+                    return None
+                if (m.in_features, m.out_features, m.weight.device) != (m0.in_features, m0.out_features, m0.weight.device):
+                    return None
+        K, inter = w1[0].in_features, w1[0].out_features
+        # w2's envelope (in_features % 128) makes inter a multiple of 128: h is quantised in 128-k groups for the down launch
+        if (w3[0].in_features, w3[0].out_features) != (K, inter) or w2[0].in_features != inter:
+            return None
+        out = {"fp8blk": True}
+        for name, mods in (("w1", w1), ("w3", w3), ("w2", w2)):
+            weight = torch.stack([m.weight.view(torch.uint8) for m in mods]).view(torch.float8_e4m3fn)
+            scale = torch.stack([m.weight_scale_inv for m in mods]).contiguous()
+            for e, m in enumerate(mods):  # the modules keep working on their own; no second copy of the weights
+                m.weight = weight[e]
+                if scale[e].data_ptr() % 16 == 0:  # the layer kernel wants 16-byte aligned scales (a few bytes each)
+                    m.weight_scale_inv = scale[e]
+            out[name] = dict(weight=weight, scale=scale, K=mods[0].in_features, N=mods[0].out_features)
+        return out
+
+    def _forward_grouped_fp8blk(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
+        """Block-FP8 experts: align -> gather-and-quantise -> gate|up -> quantise h -> down -> combine (include/b2q.h)."""
+        from ._lib import check, lib
+
+        if x.dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError(f"MoEExperts: block-FP8 experts take fp16 / bf16 activations, got {x.dtype}")
+        T, top_k = topk_ids.shape
+        rows, E = T * top_k, self.num_experts
+        dev, dt = x.device, x.dtype
+        code = 0 if dt == torch.float16 else 1
+        s1, s3, s2 = self._stack["w1"], self._stack["w3"], self._stack["w2"]
+        K, inter, Kout = s1["K"], s1["N"], s2["N"]
+        # the gather kernel reads x [T, K] by token index: a mismatched x would be read out of bounds
+        if tuple(x.shape) != (T, K) or dev != s1["weight"].device or tuple(topk_weights.shape) != (T, top_k):
+            raise ValueError(f"MoEExperts: x {tuple(x.shape)} on {dev} does not fit [{T}, {K}] on {s1['weight'].device}, "
+                             f"or topk_weights {tuple(topk_weights.shape)} is not [{T}, {top_k}]")
+        st = torch.cuda.current_stream(dev).cuda_stream
+        ids = topk_ids.to(torch.int32).contiguous()
+        wts = topk_weights.to(torch.float32).contiguous()
+        x2 = x.contiguous()
+        if x2.data_ptr() % 16 != 0:
+            x2 = x2.clone()
+        p = lambda t: t.data_ptr()  # noqa: E731
+        mp = (rows + 3) // 4 * 4  # token-scale row length of the quantiser's [K/128, Mp] layout
+        tables = torch.empty(2 * E + rows, dtype=torch.int32, device=dev)
+        counts, offsets, sorted_pairs = tables[:E], tables[E:2 * E], tables[2 * E:]
+        codes = torch.empty((rows, K), dtype=torch.uint8, device=dev)
+        s_x = torch.empty((K // 128, mp), dtype=torch.float32, device=dev)
+        h = torch.empty((rows, inter), dtype=dt, device=dev)
+        codes_h = torch.empty((rows, inter), dtype=torch.uint8, device=dev)
+        s_h = torch.empty((inter // 128, mp), dtype=torch.float32, device=dev)
+        ypair = torch.empty((rows, Kout), dtype=torch.float32, device=dev)
+        y = torch.empty((T, Kout), dtype=dt, device=dev)
+        active = min(E, rows)
+        check(lib.b2q_moe_align(p(ids), T, top_k, E, p(counts), p(offsets), p(sorted_pairs), st), "b2q_moe_align")
+        check(lib.b2q_fp8blk_moe_gather(p(x2), p(sorted_pairs), p(codes), p(s_x), T, top_k, K, code, st),
+              "b2q_fp8blk_moe_gather")
+        check(lib.b2q_fp8blk_moe_gate_up(p(codes), p(s_x), p(s1["weight"]), p(s1["scale"]), p(s3["weight"]),
+                                         p(s3["scale"]), p(h), p(counts), p(offsets), E, rows, active, K, inter, code, 0,
+                                         st), "b2q_fp8blk_moe_gate_up")
+        check(lib.b2q_fp8blk_quantize(p(h), p(codes_h), p(s_h), rows, inter, code, st), "b2q_fp8blk_quantize")
+        check(lib.b2q_fp8blk_moe_down(p(codes_h), p(s_h), p(s2["weight"]), p(s2["scale"]), p(counts), p(offsets),
+                                      p(sorted_pairs), p(wts), p(ypair), E, rows, active, inter, Kout, code, 0, st),
+              "b2q_fp8blk_moe_down")
+        check(lib.b2q_moe_combine(p(ypair), p(y), T, top_k, Kout, code, st), "b2q_moe_combine")
+        return y
 
     @staticmethod
     def _kernel_zeros(m):
@@ -222,7 +304,10 @@ class MoEExperts(torch.nn.Module):
         """x [T, K]; topk_ids / topk_weights [T, top_k] (weights already normalised) -> [T, K_out] (all-reduced)."""
         T, top_k = topk_ids.shape
         if self._stack is not None and x.is_cuda and x.dim() == 2:
-            out = self._forward_grouped(x, topk_ids, topk_weights)
+            if "fp8blk" in self._stack:
+                out = self._forward_grouped_fp8blk(x, topk_ids, topk_weights)
+            else:
+                out = self._forward_grouped(x, topk_ids, topk_weights)
             if self.reduce is not None and out.numel() <= self.reduce.max_elems and out.numel() % 8 == 0:
                 return self.reduce(out.contiguous())
             return tp.all_reduce_sum_(out, self.group)

@@ -288,6 +288,34 @@ int b2q_fp8blk_mm(const void* codes, const float* s_x, const void* weight, const
 int b2q_fp8blk_forward(const void* x, const void* weight, const float* s_w, const void* bias, void* out, int M, int K,
                        int N, int dtype, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Block-FP8 MoE experts (an addition to ABI v8): the experts' w1 / w3 [E*I, K], w2 [E*H, I] e4m3 stacks and their scale
+ * stacks [E, ceil(N/128), K/128] (each expert's checkpoint tensors, back to back), the routing tables of b2q_moe_align.
+ * One block is six launches with no host synchronisation: b2q_moe_align, b2q_fp8blk_moe_gather, b2q_fp8blk_moe_gate_up,
+ * b2q_fp8blk_quantize of h, b2q_fp8blk_moe_down, b2q_moe_combine.  For every routed pair (token t, slot j, expert e),
+ * with Q the quantiser and the promotion chain of b2q_fp8blk_mm above:
+ *   (c, s_x)  = Q(x_t)                           (the codes b2q_fp8blk_quantize gives the token)
+ *   g = T(chain(c, s_x, W1_e)),  u = T(chain(c, s_x, W3_e))
+ *   a = T(silu(g)) (silu(g) = g / (1 + __expf(-g)) in fp32),  h = T(a * u)
+ *   (c_h, s_h) = Q(h)                            (down_proj quantises its own input, as transformers' FP8Linear)
+ *   yp_j = T(chain(c_h, s_h, W2_e))
+ *   y_t  = T(sum_j fp32(w_j * yp_j))             (fp32, slot order, one rounding: b2q_moe_combine)
+ * These are the rounding points of transformers' per-expert FP8Linear loop.  Each expert's rows run the dense kernel's
+ * promotion chain and split-K rank order, so for a pinned ks the grouped results equal b2q_fp8blk_mm on that expert's
+ * rows.  Envelope: K % 128 == 0, N % 64 == 0 (the h width I of gate|up also % 128 for its quantiser), E <= 256,
+ * ks <= 8, pointers as for b2q_fp8blk_mm. */
+/* codes e4m3 [T*top_k, K], s_x fp32 [K/128, Mp(T*top_k)]: sorted row i = Q(x[sorted_pairs[i] / top_k]). */
+int b2q_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* codes, float* s_x, int T, int top_k, int K,
+                          int dtype, void* stream);
+/* h T [rows, N]: w1 / w3 [E*N, K], N = the intermediate size; active = experts expected to hold rows (grid sizing). */
+int b2q_fp8blk_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                           const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                           int active, int K, int N, int dtype, int ks, void* stream);
+/* ypair fp32 [rows, N]: row pair = w[pair] * yp of sorted row i, pair = sorted_pairs[i]; w2 [E*N, K], K = the
+ * intermediate size. */
+int b2q_fp8blk_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                        const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                        int E, int rows, int active, int K, int N, int dtype, int ks, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
