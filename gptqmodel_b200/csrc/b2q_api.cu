@@ -4,6 +4,7 @@
 #include <cstdlib>
 
 #include "../../include/b2q.h"
+#include "b2q_gemm.cuh"
 #include "b2q_internal.h"
 
 namespace b2q {
@@ -95,8 +96,10 @@ static int validate(const char* fn, const void* x, const void* packed, const voi
     set_error("%s: shape M=%d K=%d N=%d not supported (K multiple of 64, N multiple of 32)", fn, M, K, N);
     return -2;
   }
-  if (group_size < 32 || group_size % 32 != 0 || K % group_size != 0) {
-    set_error("%s: group_size=%d not supported for K=%d (multiple of 32 dividing K)", fn, group_size, K);
+  // the tensor-core tiers index scale rows by log2(32-k chunks per group) and treat any other size as per-channel
+  // (gemm_gshc): a group of 96 or 256 would read group 0's scales for every k
+  if (!((group_size == 32 || group_size == 64 || group_size == 128) && K % group_size == 0) && group_size != K) {
+    set_error("%s: group_size=%d not supported for K=%d (32 | 64 | 128 dividing K, or K)", fn, group_size, K);
     return -2;
   }
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
@@ -739,8 +742,12 @@ int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const vo
                    const int* N, int M, int K, int bits, int group_size, int dtype, void* workspace,
                    size_t workspace_bytes, void* stream) {
   if (x == nullptr || packed == nullptr || scales == nullptr || qzeros == nullptr || bias == nullptr ||
-      out == nullptr || N == nullptr || nsets < 1) {
+      out == nullptr || N == nullptr) {
     set_error("b2q_gemm_multi: null pointer argument");
+    return -2;
+  }
+  if (nsets < 1 || nsets > G_MAX_SETS) {
+    set_error("b2q_gemm_multi: nsets=%d out of range (1..%d)", nsets, G_MAX_SETS);
     return -2;
   }
   int v = validate("b2q_gemm_multi", x, packed[0], scales[0], out[0], M, K, N[0], bits, group_size, dtype);
@@ -748,6 +755,15 @@ int b2q_gemm_multi(const void* x, int nsets, const void* const* packed, const vo
   if (bits != 4 || M <= 128) {
     set_error("b2q_gemm_multi: the fused prefill launch serves bits=4, M > 128 (got bits=%d M=%d)", bits, M);
     return -2;
+  }
+  for (int i = 1; i < nsets; ++i) {
+    if (N[i] <= 0 || N[i] % 32 != 0 || packed[i] == nullptr || scales[i] == nullptr || out[i] == nullptr ||
+        ((qzeros[i] != nullptr) != (qzeros[0] != nullptr)) || (reinterpret_cast<uintptr_t>(packed[i]) & 15) ||
+        (reinterpret_cast<uintptr_t>(out[i]) & 15)) {
+      set_error("b2q_gemm_multi: set %d unsupported (N=%d; all sets share K, group size and symmetry, packed and out "
+                "16-byte aligned)", i, N[i]);
+      return -2;
+    }
   }
   DeviceGuard dg(packed[0]);
   MmArgs a = make_args(x, packed[0], scales[0], qzeros[0], perm, bias[0], out[0], M, K, N[0], bits, group_size, dtype,

@@ -366,26 +366,14 @@ static int launch_gemm_sets(const MmArgs& a, const void* x, const GemmSets& S) {
 #undef B2Q_GEMM_CASE
 }
 
-// Sibling QuantLinears in one launch (b2q_gemm_multi); x = activations with act-order already applied
+// Sibling QuantLinears in one launch (b2q_gemm_multi); x = activations with act-order already applied.  The sets were
+// validated by the caller (b2q_gemm_multi / b2q_gemm) before any CUDA work.
 int launch_gemm_multi(const MmArgs& a, const void* x, int nsets, const void* const* packed, const void* const* scales,
                       const int32_t* const* qzeros, const void* const* bias, void* const* out, const int* Ns) {
-  if (nsets < 1 || nsets > G_MAX_SETS) {
-    set_error("b2q_gemm_multi: nsets=%d out of range (1..%d)", nsets, G_MAX_SETS);
-    return -1;
-  }
-  if (a.K % G_BK != 0) {
-    set_error("b2q_gemm_multi: K=%d must be a multiple of %d", a.K, G_BK);
-    return -1;
-  }
   GemmSets S = {};
   S.nsets = nsets;
   int tn = 0;
   for (int i = 0; i < nsets; ++i) {
-    if (Ns[i] <= 0 || Ns[i] % 32 != 0 || packed[i] == nullptr || scales[i] == nullptr || out[i] == nullptr ||
-        ((qzeros[i] != nullptr) != (qzeros[0] != nullptr))) {
-      set_error("b2q_gemm_multi: set %d unsupported (N=%d; all sets share K, group size and symmetry)", i, Ns[i]);
-      return -1;
-    }
     tn += (Ns[i] + G_BN - 1) / G_BN;
     S.tn_end[i] = tn;
     S.N[i] = Ns[i];

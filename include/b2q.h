@@ -63,7 +63,8 @@ int b2q_prepack(const int32_t* qweight, const int32_t* perm, void* packed, int K
  *   x, scales, bias, out : fp16 (dtype 0) or bf16 (dtype 1), all the same type; x and out contiguous row-major
  *   qzeros               : NULL for symmetric layers (zero-point 2^(bits-1)), else int32 [G, N*bits/32]
  *   perm                 : NULL, or int32 [2K]: the act-order permutation used at prepack followed by its inverse
- *   group_size           : 32 | 64 | 128 | K (per-channel; the reference's -1)
+ *   group_size           : 32 | 64 | 128 | K (per-channel; the reference's -1); any other size returns -2, in every
+ *                          entry point that takes a GPTQ group size
  *   workspace            : >= b2q_workspace_bytes(M, K, N, perm != NULL) bytes, may be NULL when that is 0 */
 int b2q_mm(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
            const void* bias, void* out, int M, int K, int N, int bits, int group_size, int dtype, void* workspace,

@@ -50,6 +50,27 @@ def test_abi_argument_validation_without_gpu():
     assert g.lib.b2q_mm(one, one, one, None, None, None, one, 1, 64, 64, 4, 48, 0, None, 0, None) == -2
     assert b"group_size=48" in g.lib.b2q_last_error()
     assert g.lib.b2q_mm(one, one, one, None, None, None, one, 0, 64, 64, 4, 32, 0, None, 0, None) == 0  # M == 0
+    # group sizes: 32 | 64 | 128 dividing K, or K.  The tensor-core tiers index scale rows by log2(32-k chunks per group)
+    # and read any other size as per-channel (group 0 for every k), so e.g. g256 at K = 512 is refused by every entry
+    # point, not computed wrongly
+    vp1 = ctypes.c_void_p * 1
+    for K, gs in ((512, 256), (192, 96)):
+        calls = {
+            "b2q_mm": lambda: g.lib.b2q_mm(one, one, one, None, None, None, one, 16, K, 64, 4, gs, 0, None, 0, None),
+            "b2q_gemm": lambda: g.lib.b2q_gemm(one, one, one, None, None, None, one, 16, K, 64, 8, gs, 0, None, 0, None),
+            "b2q_gemm_multi": lambda: g.lib.b2q_gemm_multi(one, 1, vp1(16), vp1(16), vp1(None), None, vp1(None), vp1(16),
+                                                           (ctypes.c_int * 1)(64), 256, K, 4, gs, 0, None, 0, None),
+            "b2q_gemv": lambda: g.lib.b2q_gemv(one, one, one, None, None, None, one, K, 64, 8, gs, 0, 0, 0, None),
+            "b2q_moe_gate_up": lambda: g.lib.b2q_moe_gate_up(one, one, one, None, one, one, None, one, one, one, 2, 4, 2,
+                                                             K, 64, 4, gs, 0, None),
+        }
+        for fn, call in calls.items():
+            assert call() == -2, (fn, K, gs)
+            err = g.lib.b2q_last_error()
+            assert fn.encode() in err and f"group_size={gs}".encode() in err, (fn, err)
+    # per-channel: group_size == K, also when K is not a multiple of 128
+    assert g.lib.b2q_mm(one, one, one, None, None, None, one, 0, 192, 64, 4, 192, 0, None, 0, None) == 0
+    assert g.lib.b2q_mm(one, one, one, None, None, None, one, 0, 512, 64, 8, 512, 0, None, 0, None) == 0
     # b2q_gemv serves exactly the M=1 shapes of the decode tier and the 8-bit GEMV, refused before any CUDA work
     assert g.lib.b2q_gemv(one, one, one, None, None, None, one, 192, 64, 8, 64, 0, 0, 0, None) == -2  # K % 128 != 0
     assert b"no M=1 tier" in g.lib.b2q_last_error()
