@@ -33,6 +33,7 @@ SYMBOLS = {
     "b2q_decode_allreduce_flag_bytes": (_sz, []),
     "b2q_debug_decode_plan": (_i, [_i, _i, _i, _i, _i, _i, _vp]),
     "b2q_debug_decode_occupancy": (_i, [_i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_debug_wgmma_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_permute_cols": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
     "b2q_hadamard": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _vp]),
     "b2q_moe_align": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),

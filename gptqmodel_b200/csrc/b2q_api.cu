@@ -173,6 +173,27 @@ int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, i
   return 0;
 }
 
+int b2q_debug_wgmma_plan(int tier, int mode, int M, int K, int N, int active, int ks, int* out4) {
+  bool ok = out4 != nullptr && M >= 1 && K > 0 && N > 0 && active >= 0 && ks >= 0 && ks <= 8;
+  if (tier == 0) ok = ok && mode >= 0 && mode <= 2 && (mode != 0 || M <= 128) && K % 64 == 0 && N % 32 == 0;
+  else if (tier == 1) ok = ok && mode == 0 && ks == 0 && K <= 65536 && K % 64 == 0 && N % 64 == 0 && (K % 128 == 0 || N % 128 == 0);
+  else if (tier == 2) ok = ok && mode >= 0 && mode <= 2 && K <= 65536 && K % 128 == 0 && N % 64 == 0;
+  else ok = false;
+  if (!ok) {
+    set_error("b2q_debug_wgmma_plan: bad argument (tier=%d mode=%d M=%d K=%d N=%d active=%d ks=%d)", tier, mode, M, K, N,
+              active, ks);
+    return -2;
+  }
+  const SwapPlan p = tier == 0 ? midm_plan(mode, M, K, N, active, ks)
+                     : tier == 1 ? qqq_plan(M, K, N)
+                                 : fp8blk_plan(mode, M, K, N, active, ks);
+  out4[0] = p.ntok;
+  out4[1] = p.ks;
+  out4[2] = p.kpc;
+  out4[3] = p.tblocks;
+  return 0;
+}
+
 int b2q_debug_decode_occupancy(int version, int M, int K, int N, int ks, int warps, int* blocks) {
   if (blocks == nullptr || (version != 1 && version != 2) || M < 1 || M > 8 || K < 128 || K % 128 != 0 || N < 32 ||
       N % 32 != 0) {

@@ -72,6 +72,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
@@ -151,6 +154,42 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t local_saddr, uint32_t cta
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_saddr), "r"(cta));
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(ra) : "memory");
   return v;
+}
+__device__ __forceinline__ void ld_dsmem_v4(uint32_t cluster_saddr, float (&v)[4]) {
+  asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3])
+               : "r"(cluster_saddr)
+               : "memory");
+}
+__device__ __forceinline__ void ld_dsmem_v4(uint32_t cluster_saddr, int (&v)[4]) {
+  asm volatile("ld.shared::cluster.v4.s32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
+               : "r"(cluster_saddr)
+               : "memory");
+}
+// Split-K reduction of the swapped-operand wgmma tiers: NCH 4-wide chunks, `stride` bytes apart from `local` in the shared
+// memory of every rank of the cluster, each summed over ranks 0, 1, ..., nrank - 1 in that order, from zero (FROM_ZERO: a
+// float sum of zeros is +0) or from rank 0's value (a sum of -0s stays -0).  NCH 2 serves the gate|up pairs of the grouped
+// MoE mode.  One loop over all ranks: it unrolls, so the loads of several ranks are in flight at once.
+template <int NCH, bool FROM_ZERO, typename V>
+__device__ __forceinline__ void dsmem_sum4(uint32_t local, uint32_t stride, uint32_t nrank, V (&a)[NCH][4]) {
+  if (FROM_ZERO) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[c][i] = V(0);
+  }
+  for (uint32_t r = 0; r < nrank; ++r) {
+    uint32_t ra;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      V v[4];
+      ld_dsmem_v4(ra + c * stride, v);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[c][i] = (FROM_ZERO || r != 0) ? a[c][i] + v[i] : v[i];
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------

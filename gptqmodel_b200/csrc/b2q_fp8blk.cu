@@ -130,36 +130,11 @@ __global__ void __launch_bounds__(F_QUANT_THREADS)
 // ------------------------------------------------------------------------------------------------
 // GEMM
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-
-// MODE 1: h[i, c] = T(T(silu(g)) * u) with g, u the T-rounded products of w1 and w3
-template <typename T>
-__device__ __forceinline__ uint32_t fblk_silu_mul2(float g0, float g1, float u0, float u1) {
-  using E = ET<T>;
-  const float g[2] = {g0, g1}, u[2] = {u0, u1};
-  float h[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const float gq = E::to_f(E::from_f(g[i])), uq = E::to_f(E::from_f(u[i]));
-    const float aq = E::to_f(E::from_f(gq / (1.f + __expf(-gq))));
-    h[i] = aq * uq;
-  }
-  return E::pack2(h[0], h[1]);
-}
-
 // grouped launches (MODE 1 / 2) over the experts of a MoE block
 struct FblkMoeArgs {
   CUtensorMap tmap_w3;           // MODE 1: the w3 stack [E*N, K], 64-row boxes (tmap_w: the w1 stack, the same boxes)
-  const int32_t* counts;         // [E] rows of expert e
-  const int32_t* offsets;        // [E] first sorted row of expert e
-  const int32_t* sorted_pairs;   // [rows] pair index (token * top_k + j) of sorted row i   (MODE 2)
-  const float* pair_weights;     // [rows] routing weight by pair index                     (MODE 2)
+  MoeRoute route;
   const float* s_w3;             // [E, ceil(N/128), K/128] scales of w3                     (MODE 1)
-  float* ypair;                  // [rows, N] fp32, row = pair index                          (MODE 2)
-  int tblocks;                   // token blocks of NTOK rows per expert
-  int z0;                        // (expert, token block) of blockIdx.z == 0 (grids over 65535 blocks are split)
 };
 
 // the GEMM of fp8blk_gemm_kernel (MODE 0) and fp8blk_moe_gemm_kernel (MODE 1 / 2, G their grouped arguments).
@@ -188,18 +163,9 @@ __device__ __forceinline__ void fp8blk_gemm_body(const CUtensorMap& tmap_w, cons
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nt = blockIdx.x, n0 = nt * (MODE == 1 ? F_BF / 2 : F_BF);  // MODE 1: 64 gate + 64 up features
-  int row0 = blockIdx.z * NTOK;
-  int e = 0;  // expert (grouped modes)
-  if (MODE != 0) {
-    // the routing tables are the output of the preceding kernels: nothing may be read before they have finished
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int z = G->z0 + (int)blockIdx.z;
-    e = z / G->tblocks;
-    const int tb = z - e * G->tblocks, cnt = G->counts[e];
-    if (tb * NTOK >= cnt) return;  // the same decision in every CTA of the cluster (they differ in blockIdx.y only)
-    row0 = G->offsets[e] + tb * NTOK;
-    M = row0 + min(NTOK, cnt - tb * NTOK);  // the stores stop at the expert's last row
-  }
+  int row0 = blockIdx.z * NTOK, rows = min(NTOK, M - row0);  // first row and row count of this CTA's token block
+  int e = 0;                                                   // expert (grouped modes)
+  if (MODE != 0 && !moe_block<NTOK>(G->route, e, row0, rows)) return;
   const int wrow = MODE == 0 ? n0 : e * N + n0;  // first row of the tile in the (stacked) weight tensor
   const int KB = K / F_BK;
   const uint32_t nrank = cluster_nctarank(), crank = cluster_ctarank();
@@ -346,96 +312,40 @@ __device__ __forceinline__ void fp8blk_gemm_body(const CUtensorMap& tmap_w, cons
     }
     // both warpgroups are done with the stages before either overwrites them with its partial tile
     asm volatile("bar.sync 1, %0;" ::"r"(F_MMA_THREADS) : "memory");
-    // this rank's fp32 partial D[feature][token] -> part[token][feature] in its own shared memory
-#pragma unroll
-    for (int v = 0; v < C::ACC; ++v) {
-      const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
-      const int feat = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_base + (uint32_t)(tok * F_BF + feat) * 4), "f"(acc[v])
-                   : "memory");
-    }
+    // this rank's fp32 partial -> part[token][feature] in its own shared memory
+    park_partial(smem_base, wg, warp & 3, acc);
   }
   __syncwarp();
   cluster_sync_all();
   if (MODE == 1 && warp < F_MMA_THREADS / 32) {
-    // lane l: gate features 2l, 2l + 1 of the tile (columns n0 + 2l, n0 + 2l + 1 of h) and their up features at + 64;
-    // the ranks' partials added in rank order as below
-    for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M; tok += (int)nrank * (F_MMA_THREADS / 32)) {
-      const uint32_t local = smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)lane * 8;
-      float g[2], u[2];
-      for (uint32_t r = 0; r < nrank; ++r) {
-        uint32_t ra;
-        float2 vg, vu;
-        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
-        asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];" : "=f"(vg.x), "=f"(vg.y) : "r"(ra) : "memory");
-        asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];" : "=f"(vu.x), "=f"(vu.y) : "r"(ra + (F_BF / 2) * 4)
-                     : "memory");
-        if (r == 0) {
-          g[0] = vg.x, g[1] = vg.y, u[0] = vu.x, u[1] = vu.y;
-        } else {
-          g[0] += vg.x, g[1] += vg.y, u[0] += vu.x, u[1] += vu.y;
-        }
-      }
-      const uint32_t hv = out_bf16 ? fblk_silu_mul2<__nv_bfloat16>(g[0], g[1], u[0], u[1])
-                                   : fblk_silu_mul2<__half>(g[0], g[1], u[0], u[1]);
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(out) + (size_t)(row0 + tok) * N + n0 + 2 * lane) = hv;
+    // rank z reduces token rows z, z + nrank, ... , a half-warp per row: lane l holds gate features 4 (l & 15) .. + 3 of
+    // the tile (those columns of h) and their up features at + 64
+    const int hw = 2 * warp + (lane >> 4), c = lane & 15;
+    for (int tok = (int)crank + (int)nrank * hw; tok < rows; tok += (int)nrank * (2 * F_MMA_THREADS / 32)) {
+      float gu[2][4];
+      dsmem_sum4<2, false>(smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)c * 16, (F_BF / 2) * 4, nrank, gu);
+      const size_t o = (size_t)(row0 + tok) * N + n0 + 4 * c;
+      if (out_bf16) store_silu_mul4(reinterpret_cast<__nv_bfloat16*>(out) + o, gu[0], gu[1]);
+      else store_silu_mul4(reinterpret_cast<__half*>(out) + o, gu[0], gu[1]);
     }
   } else if (MODE != 1 && warp < F_MMA_THREADS / 32) {
-    // rank z reduces token rows z, z + nrank, ... : the partials of ranks 0, 1, ... added in that order
+    // rank z reduces token rows z, z + nrank, ... , a warp per row
     const int nc = n0 + lane * 4;
     if (nc < N) {
-      for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M;
-           tok += (int)nrank * (F_MMA_THREADS / 32)) {
-        const uint32_t local = smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)lane * 16;
-        float a[4];
-        for (uint32_t r = 0; r < nrank; ++r) {
-          uint32_t ra;
-          float4 v;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
-          asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
-                       : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                       : "r"(ra)
-                       : "memory");
-          if (r == 0) {
-            a[0] = v.x, a[1] = v.y, a[2] = v.z, a[3] = v.w;
-          } else {
-            a[0] += v.x, a[1] += v.y, a[2] += v.z, a[3] += v.w;
-          }
-        }
-        const size_t o = (size_t)(row0 + tok) * N + nc;
+      for (int tok = (int)crank + (int)nrank * warp; tok < rows; tok += (int)nrank * (F_MMA_THREADS / 32)) {
+        float a[1][4];
+        dsmem_sum4<1, false>(smem_base + (uint32_t)tok * (F_BF * 4) + (uint32_t)lane * 16, 0, nrank, a);
         if (MODE == 2) {
-          // T(h W2) like the module, times the routing weight, in fp32 in the pair's row: moe_combine_kernel sums the
-          // top_k rows of a token and rounds once
-          const int pair = G->sorted_pairs[row0 + tok];
-          const float w = G->pair_weights[pair];
-          float4 y;
-          if (out_bf16) {
-            y = make_float4(w * __bfloat162float(__float2bfloat16_rn(a[0])), w * __bfloat162float(__float2bfloat16_rn(a[1])),
-                            w * __bfloat162float(__float2bfloat16_rn(a[2])), w * __bfloat162float(__float2bfloat16_rn(a[3])));
-          } else {
-            y = make_float4(w * __half2float(__float2half_rn(a[0])), w * __half2float(__float2half_rn(a[1])),
-                            w * __half2float(__float2half_rn(a[2])), w * __half2float(__float2half_rn(a[3])));
-          }
-          *reinterpret_cast<float4*>(G->ypair + (size_t)pair * N + nc) = y;
-        } else if (out_bf16) {
-          __nv_bfloat16 y[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            y[e] = __float2bfloat16_rn(a[e]);
-            if (bias != nullptr)
-              y[e] = __float2bfloat16_rn(__bfloat162float(y[e]) +
-                                         __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[nc + e]));
-          }
-          *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = *reinterpret_cast<const uint2*>(y);
+          const int pair = G->route.sorted_pairs[row0 + tok];
+          float* y = G->route.ypair + (size_t)pair * N + nc;
+          if (out_bf16) store_ypair4<__nv_bfloat16>(y, G->route.pair_weights[pair], a[0]);
+          else store_ypair4<__half>(y, G->route.pair_weights[pair], a[0]);
         } else {
-          __half y[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            y[e] = __float2half_rn(a[e]);
-            if (bias != nullptr)
-              y[e] = __float2half_rn(__half2float(y[e]) + __half2float(reinterpret_cast<const __half*>(bias)[nc + e]));
-          }
-          *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out) + o) = *reinterpret_cast<const uint2*>(y);
+          const size_t o = (size_t)(row0 + tok) * N + nc;
+          if (out_bf16)
+            store_out4(reinterpret_cast<__nv_bfloat16*>(out) + o, reinterpret_cast<const __nv_bfloat16*>(bias), nc, a[0]);
+          else
+            store_out4(reinterpret_cast<__half*>(out) + o, reinterpret_cast<const __half*>(bias), nc, a[0]);
         }
       }
     }
@@ -466,61 +376,6 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-typedef CUresult (*FEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// 2-D tensor map (dim0 contiguous, rows `stride` bytes apart) with zero fill past the bounds.  Encoding costs
-// microseconds of host time: cached per thread on every argument.
-static int fblk_tmap(CUtensorMap* map, CUtensorMapDataType dt, const void* p, int dim0, int dim1, size_t stride,
-                     int box0, int box1, CUtensorMapSwizzle sw) {
-  struct Entry {
-    const void* p;
-    int dt, dim0, dim1, box0, box1, sw;
-    size_t stride;
-    CUtensorMap map;
-  };
-  constexpr int NCACHE = 32;
-  static thread_local Entry cache[NCACHE];
-  static thread_local int next = 0, filled = 0;
-  for (int i = 0; i < filled; ++i) {
-    const Entry& c = cache[i];
-    if (c.p == p && c.dt == (int)dt && c.dim0 == dim0 && c.dim1 == dim1 && c.stride == stride && c.box0 == box0 &&
-        c.box1 == box1 && c.sw == (int)sw) {
-      *map = c.map;
-      return 0;
-    }
-  }
-  static FEncodeTiledFn enc = nullptr;
-  if (enc == nullptr) {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      enc = reinterpret_cast<FEncodeTiledFn>(f);
-  }
-  if (enc == nullptr) {
-    set_error("b2q_fp8blk: cuTensorMapEncodeTiled not available from the driver");
-    return -1;
-  }
-  cuuint64_t gdim[2] = {(cuuint64_t)dim0, (cuuint64_t)dim1};
-  cuuint64_t gstride[1] = {(cuuint64_t)stride};
-  cuuint32_t boxd[2] = {(cuuint32_t)box0, (cuuint32_t)box1};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, dt, 2, const_cast<void*>(p), gdim, gstride, boxd, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("b2q_fp8blk: cuTensorMapEncodeTiled failed (%d) for %p [%d, %d] box [%d, %d]", (int)r, p, dim1, dim0,
-              box1, box0);
-    return -1;
-  }
-  Entry& e = cache[next];
-  e = {p, (int)dt, dim0, dim1, box0, box1, (int)sw, stride, *map};
-  next = (next + 1) % NCACHE;
-  if (filled < NCACHE) ++filled;
-  return 0;
-}
-
 int fp8blk_mp(int M) { return (M + 3) / 4 * 4; }
 
 int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream) {
@@ -533,55 +388,56 @@ int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, in
                        (const __nv_bfloat16*)x, (uint8_t*)codes, s_x, M, K, fp8blk_mp(M));
 }
 
-// tokens per CTA: the narrowest wgmma n that holds M, 128-token blocks beyond
-static int fblk_ntok(int M) { return M <= 8 ? 8 : M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
-
-// split-K ranks: fill the SMs with (tiles x token blocks x ranks) CTAs, at least 2 k-blocks per rank, cluster <= 8
-int fp8blk_ks(int M, int K, int N) {
-  const int KB = K / F_BK, tiles = (N + F_BF - 1) / F_BF, tblocks = (M + fblk_ntok(M) - 1) / fblk_ntok(M);
-  int ks = 1;
-  while (ks < 8 && (long long)tiles * tblocks * ks * 2 <= num_sms() && KB / (ks * 2) >= 2) ks *= 2;
-  while (ks > 1 && (ks - 1) * ((KB + ks - 1) / ks) >= KB) ks >>= 1;  // every rank needs at least one k-block
-  return ks;
+// tokens per CTA: the narrowest wgmma n that holds M, 128-token blocks beyond.  Split-K ranks: fill the SMs with
+// (tiles x token blocks x ranks) CTAs, at least 2 k-blocks per rank; a grouped launch counts the token blocks of all
+// rows or `active` experts' first blocks, whichever is more.  A pinned ks (> 0) is taken as given, untrimmed.
+SwapPlan fp8blk_plan(int mode, int M, int K, int N, int active, int ks) {
+  const int KB = K / F_BK, fb = mode == 1 ? F_BF / 2 : F_BF, tiles = (N + fb - 1) / fb;
+  SwapPlan p;
+  p.ntok = swap_ntok(M, 8, 128);
+  p.tblocks = (M + p.ntok - 1) / p.ntok;
+  if (active < 1) active = 1;
+  const long long blocks = (long long)tiles * (mode == 0 || p.tblocks > active ? p.tblocks : active);
+  p.ks = ks > 0 ? ks : trim_ranks(split_k_ranks(blocks, KB, 2), KB);
+  p.kpc = (KB + p.ks - 1) / p.ks;
+  return p;
 }
 
 template <int NTOK, int FUSED>
-static int launch_fp8blk_gemm_t(const Fp8BlkArgs& a) {
+static int launch_fp8blk_gemm_t(const Fp8BlkArgs& a, const SwapPlan& p) {
   using C = FblkCfg<NTOK>;
   const int KB = a.K / F_BK;
   CUtensorMap tw, tq, ts;
-  if (fblk_tmap(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, a.N, (size_t)a.K, F_BK, F_BF,
-                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+  if (make_tmap_2d(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, a.N, (size_t)a.K, F_BK, F_BF,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
     return -1;
   if (FUSED) {
     tq = tw;  // unused
     ts = tw;
   } else {
-    if (fblk_tmap(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
-                  CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    if (make_tmap_2d(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
+                     CU_TENSOR_MAP_SWIZZLE_128B) != 0)
       return -1;
-    if (fblk_tmap(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, NTOK, 1,
-                  CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
+    if (make_tmap_2d(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, NTOK, 1,
+                     CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
       return -1;
   }
   auto kern = fp8blk_gemm_kernel<NTOK, FUSED>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8blk")) return e;
-  const int tiles = (a.N + F_BF - 1) / F_BF, tblocks = (a.M + NTOK - 1) / NTOK;
-  const int ks = a.ks > 0 ? a.ks : fp8blk_ks(a.M, a.K, a.N);
-  const int kpc = (KB + ks - 1) / ks;
-  return launch_kernel(kern, dim3(tiles, ks, tblocks), dim3(F_THREADS, 1, 1), C::SMEM_BYTES, a.stream, ks, true, tw, tq,
-                       ts, a.x, a.s_w, a.bias, a.out, a.M, a.K, a.N, kpc, a.dtype);
+  return launch_kernel(kern, dim3((a.N + F_BF - 1) / F_BF, p.ks, p.tblocks), dim3(F_THREADS, 1, 1), C::SMEM_BYTES,
+                       a.stream, p.ks, true, tw, tq, ts, a.x, a.s_w, a.bias, a.out, a.M, a.K, a.N, p.kpc, a.dtype);
 }
 
 int launch_fp8blk_gemm(const Fp8BlkArgs& a) {
-  if (a.x != nullptr) return a.dtype == 0 ? launch_fp8blk_gemm_t<8, 1>(a) : launch_fp8blk_gemm_t<8, 2>(a);
-  switch (fblk_ntok(a.M)) {
-    case 8: return launch_fp8blk_gemm_t<8, 0>(a);
-    case 16: return launch_fp8blk_gemm_t<16, 0>(a);
-    case 32: return launch_fp8blk_gemm_t<32, 0>(a);
-    case 64: return launch_fp8blk_gemm_t<64, 0>(a);
-    default: return launch_fp8blk_gemm_t<128, 0>(a);
+  const SwapPlan p = fp8blk_plan(0, a.M, a.K, a.N, 1, a.ks);
+  if (a.x != nullptr) return a.dtype == 0 ? launch_fp8blk_gemm_t<8, 1>(a, p) : launch_fp8blk_gemm_t<8, 2>(a, p);
+  switch (p.ntok) {
+    case 8: return launch_fp8blk_gemm_t<8, 0>(a, p);
+    case 16: return launch_fp8blk_gemm_t<16, 0>(a, p);
+    case 32: return launch_fp8blk_gemm_t<32, 0>(a, p);
+    case 64: return launch_fp8blk_gemm_t<64, 0>(a, p);
+    default: return launch_fp8blk_gemm_t<128, 0>(a, p);
   }
 }
 
@@ -596,72 +452,48 @@ int launch_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* c
                        (const __nv_bfloat16*)x, sorted_pairs, (uint8_t*)codes, s_x, rows, top_k, K, fp8blk_mp(rows));
 }
 
-// split-K ranks of a grouped launch: fp8blk_ks with `active` experts' token blocks in place of the layer's
-int fp8blk_moe_ks(int rows, int K, int N, int mode, int active) {
-  const int KB = K / F_BK, tiles = (N + (mode == 1 ? F_BF / 2 : F_BF) - 1) / (mode == 1 ? F_BF / 2 : F_BF);
-  const int per = (rows + fblk_ntok(rows) - 1) / fblk_ntok(rows);  // token blocks of all rows
-  const long long blocks = (long long)tiles * (per > active ? per : active);
-  int ks = 1;
-  while (ks < 8 && blocks * ks * 2 <= num_sms() && KB / (ks * 2) >= 2) ks *= 2;
-  while (ks > 1 && (ks - 1) * ((KB + ks - 1) / ks) >= KB) ks >>= 1;  // every rank needs at least one k-block
-  return ks;
-}
-
 template <int NTOK, int MODE>
-static int launch_fp8blk_moe_t(const Fp8BlkArgs& a, const Fp8BlkMoe& g, int ks) {
+static int launch_fp8blk_moe_t(const Fp8BlkArgs& a, const Fp8BlkMoe& g, const SwapPlan& p) {
   using C = FblkCfg<NTOK, MODE>;
   const int KB = a.K / F_BK;
   const int wbox = MODE == 1 ? F_BF / 2 : F_BF;
   FblkMoeArgs G = {};
   CUtensorMap tw, tq, ts;
-  if (fblk_tmap(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
-                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+  if (make_tmap_2d(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
     return -1;
-  if (MODE == 1 && fblk_tmap(&G.tmap_w3, CU_TENSOR_MAP_DATA_TYPE_UINT8, g.w3, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
-                             CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+  if (MODE == 1 && make_tmap_2d(&G.tmap_w3, CU_TENSOR_MAP_DATA_TYPE_UINT8, g.w3, a.K, g.E * a.N, (size_t)a.K, F_BK, wbox,
+                                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
     return -1;
-  if (fblk_tmap(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
-                CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+  if (make_tmap_2d(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, F_BK, NTOK,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
     return -1;
-  if (fblk_tmap(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, C::SX_BYTES / 4, 1,
-                CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
+  if (make_tmap_2d(&ts, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.s_x, a.M, KB, (size_t)fp8blk_mp(a.M) * 4, C::SX_BYTES / 4, 1,
+                   CU_TENSOR_MAP_SWIZZLE_NONE) != 0)
     return -1;
-  G.counts = g.counts;
-  G.offsets = g.offsets;
-  G.sorted_pairs = g.sorted_pairs;
-  G.pair_weights = g.pair_weights;
+  G.route = {g.counts, g.offsets, g.sorted_pairs, g.pair_weights, g.ypair, p.tblocks, 0};
   G.s_w3 = g.s_w3;
-  G.ypair = g.ypair;
-  G.tblocks = (a.M + NTOK - 1) / NTOK;
   auto kern = fp8blk_moe_gemm_kernel<NTOK, MODE>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8blk_moe")) return e;
   const int tiles = (a.N + wbox - 1) / wbox;
-  const int kpc = (KB + ks - 1) / ks;
-  // gridDim.z is at most 65535: a larger (expert, token block) grid is issued as consecutive launches over ranges of z.
-  // They stay ordered under programmatic dependent launch: every CTA executes griddepcontrol.wait before it can exit.
-  constexpr int MAX_Z = 65535;
-  const long long total_z = (long long)g.E * G.tblocks;
-  for (long long z0 = 0; z0 < total_z; z0 += MAX_Z) {
-    G.z0 = (int)z0;
-    const int grid_z = (int)(total_z - z0 < MAX_Z ? total_z - z0 : MAX_Z);
-    const int e = launch_kernel(kern, dim3(tiles, ks, grid_z), dim3(F_THREADS, 1, 1), C::SMEM_BYTES, a.stream, ks, true,
-                                tw, tq, ts, a.s_w, a.out, a.M, a.K, a.N, kpc, a.dtype, G);
-    if (e != 0) return e;
-  }
-  return 0;
+  return launch_split_z((long long)g.E * p.tblocks, [&](int z0, int grid_z) {
+    G.route.z0 = z0;
+    return launch_kernel(kern, dim3(tiles, p.ks, grid_z), dim3(F_THREADS, 1, 1), C::SMEM_BYTES, a.stream, p.ks, true, tw,
+                         tq, ts, a.s_w, a.out, a.M, a.K, a.N, p.kpc, a.dtype, G);
+  });
 }
 
 int launch_fp8blk_moe(int mode, const Fp8BlkArgs& a, const Fp8BlkMoe& g) {
   // a pinned ks is taken as given, like b2q_fp8blk_mm's, so both run the same split
-  const int ks = a.ks > 0 ? a.ks : fp8blk_moe_ks(a.M, a.K, a.N, mode, g.active > 0 ? g.active : 1);
+  const SwapPlan p = fp8blk_plan(mode, a.M, a.K, a.N, g.active, a.ks);
 #define B2Q_FBM(MODE)                                                    \
-  switch (fblk_ntok(a.M)) {                                               \
-    case 8: return launch_fp8blk_moe_t<8, MODE>(a, g, ks);                \
-    case 16: return launch_fp8blk_moe_t<16, MODE>(a, g, ks);              \
-    case 32: return launch_fp8blk_moe_t<32, MODE>(a, g, ks);              \
-    case 64: return launch_fp8blk_moe_t<64, MODE>(a, g, ks);              \
-    default: return launch_fp8blk_moe_t<128, MODE>(a, g, ks);             \
+  switch (p.ntok) {                                                       \
+    case 8: return launch_fp8blk_moe_t<8, MODE>(a, g, p);                 \
+    case 16: return launch_fp8blk_moe_t<16, MODE>(a, g, p);               \
+    case 32: return launch_fp8blk_moe_t<32, MODE>(a, g, p);               \
+    case 64: return launch_fp8blk_moe_t<64, MODE>(a, g, p);               \
+    default: return launch_fp8blk_moe_t<128, MODE>(a, g, p);              \
   }
   if (mode == 1) B2Q_FBM(1)
   B2Q_FBM(2)

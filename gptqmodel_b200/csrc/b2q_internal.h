@@ -1,5 +1,6 @@
 // b2q_internal.h — launchers shared between the .cu translation units (not part of the public C-ABI).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -76,7 +77,6 @@ struct Fp8BlkArgs {
   cudaStream_t stream;
 };
 int fp8blk_mp(int M);  // token-scale row length: M rounded up to 4
-int fp8blk_ks(int M, int K, int N);
 int launch_fp8blk_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream);
 int launch_fp8blk_gemm(const Fp8BlkArgs& a);
 // grouped (MoE) launches of the block-FP8 GEMM: a = {codes / s_x = the expert-sorted rows [M = rows, K], weight / s_w =
@@ -107,7 +107,6 @@ int launch_gemm(const MmArgs& a);
 // small-batch tier (b2q_midm.cu): swapped wgmma operands + cluster split-K, 1 <= M <= 128, 4/8-bit, any group size;
 // x = activations with act-order already applied
 bool midm_supported(const MmArgs& a);
-int midm_ranks(int K, int N);
 int launch_midm(const MmArgs& a, const void* x);
 // grouped (MoE) launches of the small-batch tier; the routing tables live on the device (b2q_moe.cu builds them)
 struct MoeGroupedArgs {
@@ -138,6 +137,57 @@ int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts
 int launch_gemm_multi(const MmArgs& a, const void* x, int nsets, const void* const* packed, const void* const* scales,
                       const int32_t* const* qzeros, const void* const* bias, void* const* out, const int* Ns);
 int gemm_gshc(const MmArgs& a);  // log2(32-k chunks per quantisation group), 31 = per-channel
+// 2-D tensor map (dim0 contiguous, rows `stride` bytes apart, zero fill past the bounds), cached per thread on every
+// argument (b2q_gemm.cu)
+int make_tmap_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* p, int dim0, int dim1, size_t stride, int box0,
+                 int box1, CUtensorMapSwizzle sw);
+
+// ---- launch plan of the swapped-operand wgmma tiers (small-batch, QQQ, block-FP8): the weights are the wgmma A operand,
+// NTOK tokens the B operand, and the `ks` CTAs of a cluster split the k-blocks of a feature tile ----
+// tokens per CTA: the narrowest wgmma n that holds M, i.e. M rounded up to a power of two, clamped to [lo, hi]
+inline int swap_ntok(int M, int lo, int hi) {
+  int n = lo;
+  while (n < M && n < hi) n *= 2;
+  return n;
+}
+// split-K ranks: double while twice the CTAs still fit on the SMs and every rank keeps >= min_kb of the nkb k-blocks;
+// at most 8, the portable cluster size
+inline int split_k_ranks(long long ctas_per_rank, int nkb, int min_kb) {
+  int ks = 1;
+  while (ks < 8 && ctas_per_rank * ks * 2 <= num_sms() && nkb / (ks * 2) >= min_kb) ks *= 2;
+  return ks;
+}
+// halve ks until every rank owns at least one k-block
+inline int trim_ranks(int ks, int nkb) {
+  while (ks > 1 && (ks - 1) * ((nkb + ks - 1) / ks) >= nkb) ks >>= 1;
+  return ks;
+}
+struct SwapPlan {
+  int ntok;     // tokens per CTA
+  int ks;       // split-K ranks (cluster size)
+  int kpc;      // k-blocks per rank
+  int tblocks;  // token blocks (of ntok rows) of the layer, or per expert for grouped launches
+};
+// mode 0: one layer of M tokens; 1 / 2: grouped gate|up / down over M expert-sorted rows, `active` experts expected.
+// ks > 0: the B2Q_MIDM_KS override (small-batch tier, clamped to 8 and trimmed) or a pinned ks (block-FP8, taken as is).
+SwapPlan midm_plan(int mode, int M, int K, int N, int active, int ks);    // b2q_midm.cu
+SwapPlan qqq_plan(int M, int K, int N);                                   // b2q_qqq.cu
+SwapPlan fp8blk_plan(int mode, int M, int K, int N, int active, int ks);  // b2q_fp8blk.cu
+
+// gridDim.z is at most 65535 on every CUDA device: a grouped launch over more (expert, token block) pairs than that is
+// issued as consecutive launches over ranges of z, launch(z0, grid_z) each.  Chained launches stay ordered under
+// programmatic dependent launch: every CTA of a grouped kernel executes griddepcontrol.wait (the previous grid has
+// completed and its writes are visible) before it can exit, so a launch completes only after all the launches before it,
+// and the next kernel's wait on the last launch covers them all.
+template <typename Launch>
+inline int launch_split_z(long long total_z, Launch&& launch) {
+  constexpr long long MAX_Z = 65535;
+  for (long long z0 = 0; z0 < total_z; z0 += MAX_Z) {
+    const int e = launch((int)z0, (int)(total_z - z0 < MAX_Z ? total_z - z0 : MAX_Z));
+    if (e != 0) return e;
+  }
+  return 0;
+}
 int launch_allreduce(void* inout, int n, int dtype, int rank, int world, const void* const* peer_bufs,
                      size_t flag_offset, int max_elems, void* seq, cudaStream_t stream);
 void set_error(const char* fmt, ...);

@@ -46,17 +46,10 @@ constexpr int MM_RED_WARPS = 8;             // warps 0..7 reduce the split-K par
 // accumulators and stores silu(gate) * up; MODE 2 (w2 = down) scales each row by its routing weight and scatters it to the
 // row's (token, k) slot of an fp32 buffer.
 struct MoeArgs {
-  const int32_t* counts;        // [E] rows of expert e
-  const int32_t* offsets;       // [E] first row of expert e in the sorted order
-  const int32_t* sorted_pairs;  // [rows] pair index (token * top_k + j) of sorted row i            (MODE 2)
-  const float* pair_weights;    // [rows] routing weight, indexed by PAIR index                      (MODE 2)
+  MoeRoute route;
   const uint4* packed3;         // second weight set, same shapes / strides as the first             (MODE 1)
   const void* scales3;
   const uint32_t* qzeros3;
-  float* ypair;                 // [rows, N] fp32, row = pair index                                   (MODE 2)
-  int tblocks;                  // token blocks (of NTOK rows) per expert
-  int z0;                       // (expert, token block) index of blockIdx.z == 0: launch_midm_grouped splits a grid
-                                // of more than 65535 such blocks into several launches
 };
 
 template <int BITS, int NTOK, int PST, int WST, int MODE = 0>
@@ -93,14 +86,8 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
   const T* scales_b = nullptr;
   const uint32_t* qzeros_b = nullptr;
   if (MODE != 0) {
-    // the routing tables are written by the preceding kernel of the stream: nothing may be read before it has finished
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int z = G.z0 + (int)blockIdx.z;
-    const int e = z / G.tblocks, tb = z - e * G.tblocks;
-    const int cnt = G.counts[e];
-    if (tb * NTOK >= cnt) return;  // same decision in every CTA of the cluster (they differ in blockIdx.y only)
-    row0 = G.offsets[e] + tb * NTOK;
-    M = min(NTOK, cnt - tb * NTOK);
+    int e;
+    if (!moe_block<NTOK>(G.route, e, row0, M)) return;
     const size_t groups = (size_t)(K >> 5) >> gshc;  // quantisation groups along K (gshc = log2(32-k chunks per group))
     // one expert: K*N*BITS/8 bytes of codes (uint4 units), G*N scales, G*N/(32/BITS) zero words
     const size_t wstride = (size_t)K * N / (128 / BITS), sstride = (gshc >= 31 ? 1 : groups) * (size_t)N;
@@ -250,20 +237,12 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
 #pragma unroll
       for (int mb = 0; mb < 2; ++mb) wgmma_fence_regs(acc[st][mb]);
 
-    // ---- this rank's fp32 accumulator D[feature][token] -> its own shared memory, transposed: part[set][token][feature]
-    // (the stage buffers are idle now: every load was consumed by an MMA that has completed)
+    // ---- this rank's fp32 accumulators -> part[set][token][feature] in its own shared memory (the stage buffers are idle
+    // now: every load was consumed by an MMA that has completed)
 #pragma unroll
     for (int st = 0; st < NSETS; ++st)
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-        for (int v = 0; v < C::ACC; ++v) {
-          const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
-          const int feat = 64 * mb + 16 * warp + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
-          asm volatile("st.shared.f32 [%0], %1;" ::"r"(sW + (uint32_t)((st * NTOK + tok) * MM_BF + feat) * 4),
-                       "f"(acc[st][mb][v])
-                       : "memory");
-        }
+      for (int mb = 0; mb < 2; ++mb) park_partial(sW + (uint32_t)(st * NTOK * MM_BF * 4), mb, warp, acc[st][mb]);
   } else {
     // ================================ dequant warps ================================
     // The dequant warps form DQG groups of TG threads; group gq takes the pipeline iterations i = gq, gq + DQG, ...  One
@@ -422,62 +401,15 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
     const int nc = n0 + chunk * 4;
     if (nc < N) {
       for (int tok = (int)crank + (int)nrank * (t >> 5); tok < M; tok += (int)nrank * MM_RED_WARPS) {
-        const uint32_t local = sW + (uint32_t)tok * (MM_BF * 4) + (uint32_t)chunk * 16;
-        float acc[4] = {0.f, 0.f, 0.f, 0.f}, acc2[4] = {0.f, 0.f, 0.f, 0.f};
-        for (uint32_t r = 0; r < nrank; ++r) {
-          uint32_t ra;
-          float4 v;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
-          asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
-                       : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                       : "r"(ra)
-                       : "memory");
-          acc[0] += v.x;
-          acc[1] += v.y;
-          acc[2] += v.z;
-          acc[3] += v.w;
-          if (MODE == 1) {
-            asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
-                         : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                         : "r"(ra + (uint32_t)NTOK * (MM_BF * 4))
-                         : "memory");
-            acc2[0] += v.x;
-            acc2[1] += v.y;
-            acc2[2] += v.z;
-            acc2[3] += v.w;
-          }
-        }
+        float acc[NSETS][4];
+        dsmem_sum4<NSETS, true>(sW + (uint32_t)tok * (MM_BF * 4) + (uint32_t)chunk * 16, NTOK * MM_BF * 4, nrank, acc);
         if (MODE == 0) {
-          if (bias != nullptr) {
-            // reference order: round the matmul to the output dtype, then add bias (torch.py:337-342)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) acc[i] = E::to_f(E::from_f(acc[i])) + E::to_f(bias[nc + i]);
-          }
-          *reinterpret_cast<uint2*>(out + (size_t)tok * N + nc) =
-              make_uint2(E::pack2(acc[0], acc[1]), E::pack2(acc[2], acc[3]));
+          store_out4(out + (size_t)tok * N + nc, bias, nc, acc[0]);
         } else if (MODE == 1) {
-          // the per-expert module loop of the reference model rounds at every module boundary
-          // (act_fn(w1(x)) * w3(x) with 16-bit tensors): g = T(x W1), a = T(silu(g)), u = T(x W3), h = T(a * u)
-          float hv[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float gq = E::to_f(E::from_f(acc[i])), uq = E::to_f(E::from_f(acc2[i]));
-            const float aq = E::to_f(E::from_f(gq / (1.f + __expf(-gq))));
-            hv[i] = aq * uq;
-          }
-          *reinterpret_cast<uint2*>(out + (size_t)(row0 + tok) * N + nc) =
-              make_uint2(E::pack2(hv[0], hv[1]), E::pack2(hv[2], hv[3]));
+          store_silu_mul4(out + (size_t)(row0 + tok) * N + nc, acc[0], acc[NSETS - 1]);
         } else {
-          // y = T(h W2) like the module, then the routing weight; kept in fp32 in the row's (token, k) slot — the k slots
-          // of a token are summed (and rounded ONCE) by moe_combine_kernel: no atomics, deterministic
-          const int pair = G.sorted_pairs[row0 + tok];
-          const float w = G.pair_weights[pair];
-          float4 o;
-          o.x = w * E::to_f(E::from_f(acc[0]));
-          o.y = w * E::to_f(E::from_f(acc[1]));
-          o.z = w * E::to_f(E::from_f(acc[2]));
-          o.w = w * E::to_f(E::from_f(acc[3]));
-          *reinterpret_cast<float4*>(G.ypair + (size_t)pair * N + nc) = o;
+          const int pair = G.route.sorted_pairs[row0 + tok];
+          store_ypair4<T>(G.route.ypair + (size_t)pair * N + nc, G.route.pair_weights[pair], acc[0]);
         }
       }
     }
@@ -489,42 +421,42 @@ __global__ void __launch_bounds__(MM_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-int make_x_tmap_box(CUtensorMap* map, const void* x, int M, int K, int dtype, int box_rows);  // b2q_gemm.cu
-
-// split-K ranks (cluster size) for one launch: fill the SMs, keep >= 4 k-blocks per rank, portable cluster size <= 8
-int midm_ranks(int K, int N) {
+SwapPlan midm_plan(int mode, int M, int K, int N, int active, int ks) {
   const int tiles = (N + MM_BF - 1) / MM_BF, nkb = K / MM_BK;
-  int ks = 1;
-  while (ks < 8 && tiles * ks * 2 <= num_sms() && nkb / (ks * 2) >= 4) ks *= 2;
-  return ks;
+  SwapPlan p;
+  // MODE 1 holds two accumulator sets in the registers of the MMA warpgroup: blocks of at most 64 tokens
+  p.ntok = swap_ntok(M, 16, mode == 1 ? 64 : 128);
+  p.tblocks = (M + p.ntok - 1) / p.ntok;
+  // grouped: CTAs of `active` experts' first token blocks; blocks beyond an expert's count exit at once
+  if (ks <= 0) ks = split_k_ranks((long long)tiles * (mode == 0 ? 1 : (active > 0 ? active : 1)), nkb, 4);
+  p.ks = trim_ranks(ks < 8 ? ks : 8, nkb);
+  p.kpc = (nkb + p.ks - 1) / p.ks;
+  return p;
 }
 
 constexpr int MM_DQG = 4;  // dequant groups = k-blocks dequantised concurrently
 
 template <typename T, int BITS, bool ASYM, int NTOK, int PST, int WST, int MODE = 0, int DQG = MM_DQG, bool FP8 = false>
-static int launch_midm_t(const MmArgs& a, const void* x, int ks, const MoeArgs& G = MoeArgs{}, int x_rows = 0,
+static int launch_midm_t(const MmArgs& a, const void* x, const SwapPlan& p, const MoeArgs& G = MoeArgs{},
                          int grid_z = 1) {
   using C = MidCfg<BITS, NTOK, PST, WST, MODE>;
-  CUtensorMap tmap;
-  if (make_x_tmap_box(&tmap, x, MODE == 0 ? a.M : x_rows, a.K, a.dtype, NTOK) != 0) return -1;
+  CUtensorMap tmap;  // x [M, K] (grouped: all sorted rows) in boxes of 64 k x NTOK tokens
+  if (make_tmap_2d(&tmap, a.dtype == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, x, a.K, a.M,
+                   (size_t)a.K * 2, MM_BK, NTOK, CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
   auto kern = midm_kernel<T, BITS, ASYM, NTOK, PST, WST, MODE, DQG, FP8>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_midm")) return e;
-  const int nkb = a.K / MM_BK;
-  const int kpc = (nkb + ks - 1) / ks;
-  return launch_kernel(kern, dim3((a.N + MM_BF - 1) / MM_BF, ks, grid_z), dim3(MM_THREADS, 1, 1), C::SMEM_BYTES,
-                       a.stream, ks, true, tmap, (const uint4*)a.packed, (const T*)a.scales, (const uint32_t*)a.qzeros,
-                       (const T*)a.bias, (T*)a.out, a.M, a.K, a.N, gemm_gshc(a), kpc, G);
+  return launch_kernel(kern, dim3((a.N + MM_BF - 1) / MM_BF, p.ks, grid_z), dim3(MM_THREADS, 1, 1), C::SMEM_BYTES,
+                       a.stream, p.ks, true, tmap, (const uint4*)a.packed, (const T*)a.scales, (const uint32_t*)a.qzeros,
+                       (const T*)a.bias, (T*)a.out, a.M, a.K, a.N, gemm_gshc(a), p.kpc, G);
 }
 
 bool midm_supported(const MmArgs& a) { return a.M >= 1 && a.M <= 128 && a.K % MM_BK == 0 && a.N % 32 == 0; }
 
 // x: activations with act-order already applied (launch_gemm permutes into the workspace first)
 int launch_midm(const MmArgs& a, const void* x) {
-  int ks = env().midm_ks > 0 ? env().midm_ks : midm_ranks(a.K, a.N);
-  if (ks > 8) ks = 8;
-  const int nkb = a.K / MM_BK;
-  while (ks > 1 && (ks - 1) * ((nkb + ks - 1) / ks) >= nkb) ks >>= 1;  // every rank needs at least one k-block
+  const SwapPlan p = midm_plan(0, a.M, a.K, a.N, 1, env().midm_ks);
   const bool asym = a.qzeros != nullptr;
   // ring depths: BOTH must be multiples of the number of dequant groups, so that every use of a stage is served by the
   // SAME group.  mbarrier waits only distinguish the parity of a phase: with 6-stage rings and 4 groups (first version)
@@ -534,19 +466,19 @@ int launch_midm(const MmArgs& a, const void* x) {
   // .  8 dequantised stages = two per group; 4-8 packed stages (refilled by the group's own
   // leader); 4-8 activation stages in their own ring.
 #define B2Q_MM_NTOK(T, BITS, AS)                                                                  \
-  (a.M <= 16   ? launch_midm_t<T, BITS, AS, 16, (BITS == 4 ? 12 : 8), 8>(a, x, ks)                \
-   : a.M <= 32 ? launch_midm_t<T, BITS, AS, 32, (BITS == 4 ? 12 : 8), 8>(a, x, ks)                \
-   : a.M <= 64 ? launch_midm_t<T, BITS, AS, 64, (BITS == 4 ? 8 : 4), 8>(a, x, ks)                 \
-               : launch_midm_t<T, BITS, AS, 128, 4, 8>(a, x, ks))
+  (p.ntok == 16   ? launch_midm_t<T, BITS, AS, 16, (BITS == 4 ? 12 : 8), 8>(a, x, p)             \
+   : p.ntok == 32 ? launch_midm_t<T, BITS, AS, 32, (BITS == 4 ? 12 : 8), 8>(a, x, p)             \
+   : p.ntok == 64 ? launch_midm_t<T, BITS, AS, 64, (BITS == 4 ? 8 : 4), 8>(a, x, p)              \
+                  : launch_midm_t<T, BITS, AS, 128, 4, 8>(a, x, p))
 #define B2Q_MM_CASE(T)                                                          \
   (a.bits == 4 ? (asym ? B2Q_MM_NTOK(T, 4, true) : B2Q_MM_NTOK(T, 4, false))   \
                : (asym ? B2Q_MM_NTOK(T, 8, true) : B2Q_MM_NTOK(T, 8, false)))
   // FP8 layers: the 8-bit ring depths, no zero-points, the e4m3 / scale division in the dequant warps
 #define B2Q_MM_FP8(T)                                                                               \
-  (a.M <= 16   ? launch_midm_t<T, 8, false, 16, 8, 8, 0, MM_DQG, true>(a, x, ks)                    \
-   : a.M <= 32 ? launch_midm_t<T, 8, false, 32, 8, 8, 0, MM_DQG, true>(a, x, ks)                    \
-   : a.M <= 64 ? launch_midm_t<T, 8, false, 64, 4, 8, 0, MM_DQG, true>(a, x, ks)                    \
-               : launch_midm_t<T, 8, false, 128, 4, 8, 0, MM_DQG, true>(a, x, ks))
+  (p.ntok == 16   ? launch_midm_t<T, 8, false, 16, 8, 8, 0, MM_DQG, true>(a, x, p)                 \
+   : p.ntok == 32 ? launch_midm_t<T, 8, false, 32, 8, 8, 0, MM_DQG, true>(a, x, p)                 \
+   : p.ntok == 64 ? launch_midm_t<T, 8, false, 64, 4, 8, 0, MM_DQG, true>(a, x, p)                 \
+                  : launch_midm_t<T, 8, false, 128, 4, 8, 0, MM_DQG, true>(a, x, p))
   if (a.fp8) return a.dtype == 0 ? B2Q_MM_FP8(__half) : B2Q_MM_FP8(__nv_bfloat16);
   return a.dtype == 0 ? B2Q_MM_CASE(__half) : B2Q_MM_CASE(__nv_bfloat16);
 #undef B2Q_MM_FP8
@@ -558,13 +490,6 @@ int launch_midm(const MmArgs& a, const void* x) {
 // grouped launches for a MoE block (b2q_moe.cu): a = {x = expert-sorted activations [rows, K], packed / scales / qzeros =
 // the STACKED tensors of all experts (expert stride = one expert's tensor), out = h [rows, N] (mode 1), M = token-box
 // width hint (largest row count one expert is expected to get), N / K of ONE expert}
-int midm_grouped_ranks(int K, int N, int active) {
-  const int tiles = (N + MM_BF - 1) / MM_BF, nkb = K / MM_BK;
-  int ks = 1;
-  while (ks < 8 && tiles * active * ks * 2 <= num_sms() && nkb / (ks * 2) >= 4) ks *= 2;
-  return ks;
-}
-
 int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   if ((a.bits != 4 && a.bits != 8) || a.K % MM_BK != 0 || a.N % 32 != 0 || (mode != 1 && mode != 2) || g.E < 1 ||
       g.rows < 1) {
@@ -572,55 +497,32 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
               a.bits, a.K, a.N, g.E, g.rows);
     return -1;
   }
+  const SwapPlan p = midm_plan(mode, g.rows, a.K, a.N, g.active, env().midm_ks);
   MoeArgs G = {};
-  G.counts = g.counts;
-  G.offsets = g.offsets;
-  G.sorted_pairs = g.sorted_pairs;
-  G.pair_weights = g.pair_weights;
+  G.route = {g.counts, g.offsets, g.sorted_pairs, g.pair_weights, g.ypair, p.tblocks, 0};
   G.packed3 = (const uint4*)g.packed3;
   G.scales3 = g.scales3;
   G.qzeros3 = (const uint32_t*)g.qzeros3;
-  G.ypair = g.ypair;
-  // token-box width: every expert may receive up to `rows` rows; boxes of 16 serve decode-sized batches with one block
-  // per expert, larger batches take 128-row blocks (CTAs of blocks beyond an expert's count exit immediately)
-  // (mode 1 holds two accumulator sets in the registers of the MMA warpgroup: blocks of at most 64 tokens)
-  const int ntok = g.rows <= 16 ? 16 : g.rows <= 32 ? 32 : (g.rows <= 64 || mode == 1) ? 64 : 128;
-  G.tblocks = (g.rows + ntok - 1) / ntok;
-  const long long total_z = (long long)g.E * G.tblocks;
-  int ks = env().midm_ks > 0 ? env().midm_ks : midm_grouped_ranks(a.K, a.N, g.active > 0 ? g.active : 1);
-  if (ks > 8) ks = 8;
-  const int nkb = a.K / MM_BK;
-  while (ks > 1 && (ks - 1) * ((nkb + ks - 1) / ks) >= nkb) ks >>= 1;
   const bool asym = a.qzeros != nullptr;
   // packed-ring depths per token block: those of B2Q_MM_NTOK (launch_midm) for the same bit width
 #define B2Q_MG_NTOK4(T, AS, MODE)                                                            \
-  (ntok == 16   ? launch_midm_t<T, 4, AS, 16, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
-   : ntok == 32 ? launch_midm_t<T, 4, AS, 32, 12, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)    \
-   : ntok == 64 ? launch_midm_t<T, 4, AS, 64, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
-                : launch_midm_t<T, 4, AS, (MODE == 1 ? 64 : 128), (MODE == 1 ? 8 : 4), 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
+  (p.ntok == 16   ? launch_midm_t<T, 4, AS, 16, 12, 8, MODE>(a, a.x, p, G, grid_z)           \
+   : p.ntok == 32 ? launch_midm_t<T, 4, AS, 32, 12, 8, MODE>(a, a.x, p, G, grid_z)           \
+   : p.ntok == 64 ? launch_midm_t<T, 4, AS, 64, 8, 8, MODE>(a, a.x, p, G, grid_z)            \
+                  : launch_midm_t<T, 4, AS, (MODE == 1 ? 64 : 128), (MODE == 1 ? 8 : 4), 8, MODE>(a, a.x, p, G, grid_z))
 #define B2Q_MG_NTOK8(T, AS, MODE)                                                            \
-  (ntok == 16   ? launch_midm_t<T, 8, AS, 16, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
-   : ntok == 32 ? launch_midm_t<T, 8, AS, 32, 8, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
-   : ntok == 64 ? launch_midm_t<T, 8, AS, 64, 4, 8, MODE>(a, a.x, ks, G, g.rows, grid_z)     \
-                : launch_midm_t<T, 8, AS, (MODE == 1 ? 64 : 128), 4, 8, MODE>(a, a.x, ks, G, g.rows, grid_z))
+  (p.ntok == 16   ? launch_midm_t<T, 8, AS, 16, 8, 8, MODE>(a, a.x, p, G, grid_z)            \
+   : p.ntok == 32 ? launch_midm_t<T, 8, AS, 32, 8, 8, MODE>(a, a.x, p, G, grid_z)            \
+   : p.ntok == 64 ? launch_midm_t<T, 8, AS, 64, 4, 8, MODE>(a, a.x, p, G, grid_z)            \
+                  : launch_midm_t<T, 8, AS, (MODE == 1 ? 64 : 128), 4, 8, MODE>(a, a.x, p, G, grid_z))
 #define B2Q_MG_NTOK(T, AS, MODE) (a.bits == 4 ? B2Q_MG_NTOK4(T, AS, MODE) : B2Q_MG_NTOK8(T, AS, MODE))
 #define B2Q_MG_CASE(T)                                                                       \
   (mode == 1 ? (asym ? B2Q_MG_NTOK(T, true, 1) : B2Q_MG_NTOK(T, false, 1))                   \
              : (asym ? B2Q_MG_NTOK(T, true, 2) : B2Q_MG_NTOK(T, false, 2)))
-  // gridDim.z is at most 65535 on every CUDA device: a prefill chunk of a many-expert block (E = 128, top_k = 8: 8T/64
-  // token blocks per expert in MODE 1, i.e. from T = 4089 on) needs more (expert, token block) pairs than that, so the grid
-  // is issued as consecutive launches over ranges of z; a grid that fits is one launch with z0 = 0, as before.  Chained
-  // launches stay ordered under programmatic dependent launch: every CTA of MODE 1 / 2 executes griddepcontrol.wait (the
-  // previous grid has completed and its writes are visible) before it can exit, so a launch completes only after all the
-  // launches before it, and the next kernel's wait on the last launch covers them all.
-  constexpr int MAX_Z = 65535;
-  for (long long z0 = 0; z0 < total_z; z0 += MAX_Z) {
-    G.z0 = (int)z0;
-    const int grid_z = (int)(total_z - z0 < MAX_Z ? total_z - z0 : MAX_Z);
-    const int e = a.dtype == 0 ? B2Q_MG_CASE(__half) : B2Q_MG_CASE(__nv_bfloat16);
-    if (e != 0) return e;
-  }
-  return 0;
+  return launch_split_z((long long)g.E * p.tblocks, [&](int z0, int grid_z) {
+    G.route.z0 = z0;
+    return a.dtype == 0 ? B2Q_MG_CASE(__half) : B2Q_MG_CASE(__nv_bfloat16);
+  });
 #undef B2Q_MG_CASE
 #undef B2Q_MG_NTOK
 #undef B2Q_MG_NTOK8

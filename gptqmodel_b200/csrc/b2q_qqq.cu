@@ -253,17 +253,10 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
     wgmma_wait<0>();
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) wgmma_fence_regs(acc[mb]);
-    // this rank's int32 partial D[feature][token] -> part[token][feature] in its own shared memory (the stage buffers
-    // are idle: every load was consumed by an MMA that has completed)
+    // this rank's int32 partial -> part[token][feature] in its own shared memory (the stage buffers are idle: every
+    // load was consumed by an MMA that has completed)
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-      for (int v = 0; v < C::ACC; ++v) {
-        const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
-        const int feat = 64 * mb + 16 * warp + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
-        asm volatile("st.shared.s32 [%0], %1;" ::"r"(sW + (uint32_t)(tok * Q_BF + feat) * 4), "r"(acc[mb][v])
-                     : "memory");
-      }
+    for (int mb = 0; mb < 2; ++mb) park_partial(sW, mb, warp, acc[mb]);
   } else {
     // ================================ dequant warps ================================
     const int f = threadIdx.x - Q_MMA_THREADS;  // feature row of the tile
@@ -320,21 +313,8 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
     if (nc < N) {
       const float4 sc = *reinterpret_cast<const float4*>(s_channel + nc);
       for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M; tok += (int)nrank * Q_RED_WARPS) {
-        const uint32_t local = sW + (uint32_t)tok * (Q_BF * 4) + (uint32_t)chunk * 16;
-        int a[4] = {0, 0, 0, 0};
-        for (uint32_t r = 0; r < nrank; ++r) {
-          uint32_t ra;
-          int4 v;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local), "r"(r));
-          asm volatile("ld.shared::cluster.v4.s32 {%0,%1,%2,%3}, [%4];"
-                       : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-                       : "r"(ra)
-                       : "memory");
-          a[0] += v.x;
-          a[1] += v.y;
-          a[2] += v.z;
-          a[3] += v.w;
-        }
+        int a[1][4];
+        dsmem_sum4<1, true>(sW + (uint32_t)tok * (Q_BF * 4) + (uint32_t)chunk * 16, 0, nrank, a);
         const int m = row0 + tok;
         const float st = s_tok[m];
         const float scs[4] = {sc.x, sc.y, sc.z, sc.w};
@@ -342,7 +322,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           // the reference epilogue: fp32(acc) * s_channel * s_tok, rounded to fp16; then D.add_(bias)
-          y[e] = __float2half_rn(__fmul_rn(__fmul_rn(__int2float_rn(a[e]), scs[e]), st));
+          y[e] = __float2half_rn(__fmul_rn(__fmul_rn(__int2float_rn(a[0][e]), scs[e]), st));
           if (bias != nullptr) y[e] = __float2half_rn(__half2float(y[e]) + __half2float(bias[nc + e]));
         }
         if (out_bf16) {
@@ -365,62 +345,6 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-typedef CUresult (*QEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// Tensor map of the codes [M, Kp] int8 for boxes of 128 k x `box` tokens, SWIZZLE_128B; rows >= M are zero-filled.
-// Encoding costs microseconds of host time: cached per thread on (pointer, M, Kp, box).
-static int make_q_tmap(CUtensorMap* map, const void* q, int M, int Kp, int box) {
-  struct Entry {
-    const void* q;
-    int M, Kp, box;
-    CUtensorMap map;
-  };
-  constexpr int NCACHE = 16;
-  static thread_local Entry cache[NCACHE];
-  static thread_local int next = 0, filled = 0;
-  for (int i = 0; i < filled; ++i) {
-    const Entry& c = cache[i];
-    if (c.q == q && c.M == M && c.Kp == Kp && c.box == box) {
-      *map = c.map;
-      return 0;
-    }
-  }
-  static QEncodeTiledFn enc = nullptr;
-  if (enc == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      enc = reinterpret_cast<QEncodeTiledFn>(p);
-  }
-  if (enc == nullptr) {
-    set_error("b2q_qqq: cuTensorMapEncodeTiled not available from the driver");
-    return -1;
-  }
-  cuuint64_t gdim[2] = {(cuuint64_t)Kp, (cuuint64_t)M};
-  cuuint64_t gstride[1] = {(cuuint64_t)Kp};
-  cuuint32_t boxd[2] = {(cuuint32_t)Q_BK, (cuuint32_t)box};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(q), gdim, gstride, boxd, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("b2q_qqq: cuTensorMapEncodeTiled failed (%d) for codes=%p M=%d Kp=%d box=%d", (int)r, q, M, Kp, box);
-    return -1;
-  }
-  Entry& e = cache[next];
-  e.q = q;
-  e.M = M;
-  e.Kp = Kp;
-  e.box = box;
-  e.map = *map;
-  next = (next + 1) % NCACHE;
-  if (filled < NCACHE) ++filled;
-  return 0;
-}
-
 int launch_qqq_quant(const void* x, void* q, float* s_tok, int M, int K, int dtype, cudaStream_t stream) {
   const int Kp = (K + Q_BK - 1) / Q_BK * Q_BK;
   if (dtype == 0)
@@ -438,37 +362,43 @@ int launch_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int gro
   return (int)cudaGetLastError();
 }
 
-// tokens per CTA: the narrowest wgmma n that holds M (decode wastes no MMA width), 128-token blocks beyond
-int qqq_ntok(int M) { return M <= 8 ? 8 : M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
+// tokens per CTA: the narrowest wgmma n that holds M (decode wastes no MMA width), 128-token blocks beyond; split-K over
+// (tiles x token blocks) CTAs, at least 2 k-blocks per rank
+SwapPlan qqq_plan(int M, int K, int N) {
+  const int KB = (K + Q_BK - 1) / Q_BK, tiles = (N + Q_BF - 1) / Q_BF;
+  SwapPlan p;
+  p.ntok = swap_ntok(M, 8, 128);
+  p.tblocks = (M + p.ntok - 1) / p.ntok;
+  p.ks = trim_ranks(split_k_ranks((long long)tiles * p.tblocks, KB, 2), KB);
+  p.kpc = (KB + p.ks - 1) / p.ks;
+  return p;
+}
 
 template <int NTOK, bool GROUPED>
-static int launch_qqq_gemm_t(const QqqArgs& a) {
+static int launch_qqq_gemm_t(const QqqArgs& a, const SwapPlan& p) {
   using C = QqqCfg<NTOK>;
   const int KB = (a.K + Q_BK - 1) / Q_BK;
-  CUtensorMap tmap;
-  if (make_q_tmap(&tmap, a.q, a.M, KB * Q_BK, NTOK) != 0) return -1;
+  CUtensorMap tmap;  // the codes [M, Kp] in boxes of 128 k x NTOK tokens; rows >= M are zero-filled
+  if (make_tmap_2d(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.q, KB * Q_BK, a.M, (size_t)KB * Q_BK, Q_BK, NTOK,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
   auto kern = qqq_gemm_kernel<NTOK, GROUPED>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_qqq")) return e;
-  // split-K ranks: fill the SMs with (tiles x token blocks x ranks) CTAs, at least 2 k-blocks per rank, cluster <= 8
-  const int tiles = (a.N + Q_BF - 1) / Q_BF, tblocks = (a.M + NTOK - 1) / NTOK;
-  int ks = 1;
-  while (ks < 8 && (long long)tiles * tblocks * ks * 2 <= num_sms() && KB / (ks * 2) >= 2) ks *= 2;
-  while (ks > 1 && (ks - 1) * ((KB + ks - 1) / ks) >= KB) ks >>= 1;  // every rank needs at least one k-block
-  const int kpc = (KB + ks - 1) / ks;
-  return launch_kernel(kern, dim3(tiles, ks, tblocks), dim3(Q_THREADS, 1, 1), C::SMEM_BYTES, a.stream, ks, true, tmap,
-                       (const uint4*)a.packed, a.s_channel, (const __half*)a.s_group, a.s_tok, (const __half*)a.bias,
-                       a.out, a.M, KB, a.N, kpc, a.out_dtype);
+  return launch_kernel(kern, dim3((a.N + Q_BF - 1) / Q_BF, p.ks, p.tblocks), dim3(Q_THREADS, 1, 1), C::SMEM_BYTES,
+                       a.stream, p.ks, true, tmap, (const uint4*)a.packed, a.s_channel, (const __half*)a.s_group,
+                       a.s_tok, (const __half*)a.bias, a.out, a.M, KB, a.N, p.kpc, a.out_dtype);
 }
 
 int launch_qqq_gemm(const QqqArgs& a) {
   const bool g = a.s_group != nullptr;
-  switch (qqq_ntok(a.M)) {
-    case 8: return g ? launch_qqq_gemm_t<8, true>(a) : launch_qqq_gemm_t<8, false>(a);
-    case 16: return g ? launch_qqq_gemm_t<16, true>(a) : launch_qqq_gemm_t<16, false>(a);
-    case 32: return g ? launch_qqq_gemm_t<32, true>(a) : launch_qqq_gemm_t<32, false>(a);
-    case 64: return g ? launch_qqq_gemm_t<64, true>(a) : launch_qqq_gemm_t<64, false>(a);
-    default: return g ? launch_qqq_gemm_t<128, true>(a) : launch_qqq_gemm_t<128, false>(a);
+  const SwapPlan p = qqq_plan(a.M, a.K, a.N);
+  switch (p.ntok) {
+    case 8: return g ? launch_qqq_gemm_t<8, true>(a, p) : launch_qqq_gemm_t<8, false>(a, p);
+    case 16: return g ? launch_qqq_gemm_t<16, true>(a, p) : launch_qqq_gemm_t<16, false>(a, p);
+    case 32: return g ? launch_qqq_gemm_t<32, true>(a, p) : launch_qqq_gemm_t<32, false>(a, p);
+    case 64: return g ? launch_qqq_gemm_t<64, true>(a, p) : launch_qqq_gemm_t<64, false>(a, p);
+    default: return g ? launch_qqq_gemm_t<128, true>(a, p) : launch_qqq_gemm_t<128, false>(a, p);
   }
 }
 

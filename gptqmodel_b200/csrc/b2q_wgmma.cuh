@@ -229,4 +229,87 @@ __device__ __forceinline__ void wgmma_fence_regs(int (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
+// ------------------------------------------------------------------------------------------------
+// shared epilogue of the swapped-operand tiers (b2q_midm.cu, b2q_qqq.cu, b2q_fp8blk.cu): the weights are the A operand,
+// so D[feature][token] is parked transposed, part[token][128 features], for the split-K reduction (dsmem_sum4)
+// ------------------------------------------------------------------------------------------------
+// the m64 x NTOK fragment d (NTOK / 2 registers, layout above) of feature block mb of the tile, by warp (w & 3) of its
+// warpgroup, into part at shared address `part`
+__device__ __forceinline__ void st_shared_4b(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_4b(uint32_t addr, int v) {
+  asm volatile("st.shared.s32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+template <int R, typename V>
+__device__ __forceinline__ void park_partial(uint32_t part, int mb, int w, const V (&d)[R]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int v = 0; v < R; ++v) {
+    const int j = v >> 2, h = (v >> 1) & 1, c = v & 1;
+    const int feat = 64 * mb + 16 * w + (lane >> 2) + 8 * h, tok = 8 * j + 2 * (lane & 3) + c;
+    st_shared_4b(part + (uint32_t)(tok * 128 + feat) * 4, d[v]);
+  }
+}
+
+// Grouped launches over the experts of a MoE block (MODE 1 = gate|up, 2 = down): z0 + blockIdx.z = (expert, token block)
+// over the expert-sorted rows that b2q_moe_align ordered; the rows of an expert are contiguous.
+struct MoeRoute {
+  const int32_t* counts;        // [E] rows of expert e
+  const int32_t* offsets;       // [E] first sorted row of expert e
+  const int32_t* sorted_pairs;  // [rows] pair index (token * top_k + j) of sorted row i   (MODE 2)
+  const float* pair_weights;    // [rows] routing weight, indexed by pair index           (MODE 2)
+  float* ypair;                 // [rows, N] fp32, row = pair index                         (MODE 2)
+  int tblocks;                  // token blocks (of NTOK rows) per expert
+  int z0;                       // (expert, token block) of blockIdx.z == 0 (launch_split_z)
+};
+// Waits for the routing tables (the output of the preceding kernels: nothing may be read before they have finished) and
+// returns false for a block past its expert's rows — the same decision in every CTA of a cluster, which differ in
+// blockIdx.y only.  Else e = the expert, row0 = the block's first sorted row, rows = its row count (<= NTOK).
+template <int NTOK>
+__device__ __forceinline__ bool moe_block(const MoeRoute& R, int& e, int& row0, int& rows) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const int z = R.z0 + (int)blockIdx.z;
+  e = z / R.tblocks;
+  const int tb = z - e * R.tblocks, cnt = R.counts[e];
+  if (tb * NTOK >= cnt) return false;
+  row0 = R.offsets[e] + tb * NTOK;
+  rows = min(NTOK, cnt - tb * NTOK);
+  return true;
+}
+
+// four consecutive outputs: T(acc), or T(T(acc) + bias) in the reference order (round the matmul to the output dtype,
+// then add bias: torch.py:337-342) of features nc .. nc + 3; bias = [N] or nullptr
+template <typename T>
+__device__ __forceinline__ void store_out4(T* dst, const T* bias, int nc, float (&a)[4]) {
+  using E = ET<T>;
+  if (bias != nullptr) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[i] = E::to_f(E::from_f(a[i])) + E::to_f(bias[nc + i]);
+  }
+  *reinterpret_cast<uint2*>(dst) = make_uint2(E::pack2(a[0], a[1]), E::pack2(a[2], a[3]));
+}
+// MODE 1: the per-expert module loop of the reference model rounds at every module boundary (act_fn(w1(x)) * w3(x) with
+// 16-bit tensors): g = T(x W1), a = T(silu(g)), u = T(x W3), h = T(a * u)
+template <typename T>
+__device__ __forceinline__ void store_silu_mul4(T* dst, const float (&g)[4], const float (&u)[4]) {
+  using E = ET<T>;
+  float h[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float gq = E::to_f(E::from_f(g[i])), uq = E::to_f(E::from_f(u[i]));
+    const float aq = E::to_f(E::from_f(gq / (1.f + __expf(-gq))));
+    h[i] = aq * uq;
+  }
+  *reinterpret_cast<uint2*>(dst) = make_uint2(E::pack2(h[0], h[1]), E::pack2(h[2], h[3]));
+}
+// MODE 2: y = T(h W2) like the module, times the routing weight, kept in fp32 in the pair's row of ypair — the top_k rows
+// of a token are summed (and rounded ONCE) by moe_combine_kernel: no atomics, deterministic
+template <typename T>
+__device__ __forceinline__ void store_ypair4(float* dst, float w, const float (&a)[4]) {
+  using E = ET<T>;
+  *reinterpret_cast<float4*>(dst) = make_float4(w * E::to_f(E::from_f(a[0])), w * E::to_f(E::from_f(a[1])),
+                                                w * E::to_f(E::from_f(a[2])), w * E::to_f(E::from_f(a[3])));
+}
+
 }  // namespace b2q

@@ -195,6 +195,14 @@ void b2q_debug_reload_env(void);
  * tiles (32 features) per group, ring stages, dynamic shared memory bytes}.  ks / warps <= 0 = heuristic. */
 int b2q_debug_decode_plan(int version, int M, int K, int N, int ks, int warps, int* out8);
 
+/* Debug / tests (host only, no GPU needed): the launch plan of a swapped-operand wgmma tier, computed by the code its
+ * launcher runs.  tier 0 = the small-batch tier of b2q_mm / b2q_moe_gate_up / b2q_moe_down, 1 = QQQ (b2q_qqq_mm),
+ * 2 = block-FP8 (b2q_fp8blk_mm / _forward / _moe_gate_up / _moe_down).  mode 0 = one layer of M tokens (tier 0: M <= 128);
+ * 1 / 2 = grouped gate|up / down over M expert-sorted rows with `active` experts expected (tiers 0 and 2).  ks > 0: the
+ * B2Q_MIDM_KS override (tier 0) or a pinned ks (tier 2); tier 1 takes none.  Shapes as the tier's entry points accept them.
+ * out4 = {tokens per CTA, split-K ranks, k-blocks per rank, token blocks}.  Bad arguments return -2. */
+int b2q_debug_wgmma_plan(int tier, int mode, int M, int K, int N, int active, int ks, int* out4);
+
 /* Resident CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor on the current device) of the fp16, symmetric,
  * group-128 instantiation of decode kernel `version`, at the block size and dynamic shared memory of the plan
  * b2q_debug_decode_plan returns for the same arguments. */
