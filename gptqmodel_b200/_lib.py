@@ -60,6 +60,12 @@ SYMBOLS = {
     "b2q_fp8blk_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_qqq_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b2q_qqq_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i,
+                                 _vp]),
+    "b2q_qqq_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

@@ -488,6 +488,91 @@ int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, c
                 (cudaStream_t)stream);
 }
 
+// ---- QQQ MoE experts: the grouped modes of qqq_gemm_kernel over the routing tables of b2q_moe_align ----
+int b2q_qqq_moe_gather(const void* x, const int32_t* sorted_pairs, int8_t* q, float* s_tok, int T, int top_k, int K,
+                       int dtype, void* stream) {
+  if (T < 1 || top_k < 1 || K <= 0 || K % 64 != 0 || K > 65536) {
+    set_error("b2q_qqq_moe_gather: T=%d, top_k=%d must be >= 1 and K=%d a multiple of 64 <= 65536", T, top_k, K);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("b2q_qqq_moe_gather: dtype=%d not supported (0 fp16, 1 bf16)", dtype);
+    return -2;
+  }
+  if (x == nullptr || sorted_pairs == nullptr || q == nullptr || s_tok == nullptr || !aligned16(x) || !aligned16(q)) {
+    set_error("b2q_qqq_moe_gather: x, sorted_pairs, q and s_tok must be device pointers, x and q 16-byte aligned");
+    return -2;
+  }
+  DeviceGuard dg(q);
+  return check_cuda(launch_qqq_moe_gather(x, sorted_pairs, q, s_tok, T * top_k, top_k, K, dtype, (cudaStream_t)stream),
+                    "b2q_qqq_moe_gather");
+}
+
+static int qqq_moe_check(const char* fn, const int8_t* q, const float* s_tok, const void* packed,
+                         const float* s_channel, const void* s_group, void* out, const int32_t* counts,
+                         const int32_t* offsets, int E, int rows, int K, int N, int group_size, int dtype) {
+  if (int e = qqq_check_mm(fn, packed, s_channel, s_group, out, rows, K, N, group_size, dtype)) return e;
+  if (q == nullptr || s_tok == nullptr || counts == nullptr || offsets == nullptr || !aligned16(q)) {
+    set_error("%s: q, s_tok, counts and offsets must be device pointers, q 16-byte aligned", fn);
+    return -2;
+  }
+  if (E < 1 || E > 256 || rows < 1) {
+    set_error("%s: E=%d (1..256), rows=%d (>= 1) outside the envelope", fn, E, rows);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_qqq_moe_gate_up(const int8_t* q, const float* s_tok, const void* packed1, const float* s_channel1,
+                        const void* s_group1, const void* packed3, const float* s_channel3, const void* s_group3, void* h,
+                        const int32_t* counts, const int32_t* offsets, int E, int rows, int active, int K, int N,
+                        int group_size, int dtype, void* stream) {
+  if (int e = qqq_moe_check("b2q_qqq_moe_gate_up", q, s_tok, packed1, s_channel1, s_group1, h, counts, offsets, E, rows,
+                            K, N, group_size, dtype))
+    return e;
+  if (int e = qqq_check_mm("b2q_qqq_moe_gate_up", packed3, s_channel3, s_group3, h, rows, K, N, group_size, dtype))
+    return e;
+  if (N % 64 != 0) {
+    set_error("b2q_qqq_moe_gate_up: N=%d must be a multiple of 64 (64 gate + 64 up features per tile)", N);
+    return -2;
+  }
+  DeviceGuard dg(packed1);
+  QqqArgs a = {q, s_tok, packed1, s_channel1, s_group1, nullptr, h, rows, K, N, dtype, (cudaStream_t)stream};
+  QqqMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.packed3 = packed3;
+  g.s_channel3 = s_channel3;
+  g.s_group3 = s_group3;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_qqq_moe(1, a, g), "b2q_qqq_moe_gate_up");
+}
+
+int b2q_qqq_moe_down(const int8_t* q_h, const float* s_h, const void* packed2, const float* s_channel2,
+                     const void* s_group2, const int32_t* counts, const int32_t* offsets, const int32_t* sorted_pairs,
+                     const float* pair_weights, float* ypair, int E, int rows, int active, int K, int N, int group_size,
+                     int dtype, void* stream) {
+  if (int e = qqq_moe_check("b2q_qqq_moe_down", q_h, s_h, packed2, s_channel2, s_group2, ypair, counts, offsets, E, rows,
+                            K, N, group_size, dtype))
+    return e;
+  if (sorted_pairs == nullptr || pair_weights == nullptr) {
+    set_error("b2q_qqq_moe_down: sorted_pairs and pair_weights must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(packed2);
+  QqqArgs a = {q_h, s_h, packed2, s_channel2, s_group2, nullptr, ypair, rows, K, N, dtype, (cudaStream_t)stream};
+  QqqMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.sorted_pairs = sorted_pairs;
+  g.pair_weights = pair_weights;
+  g.ypair = ypair;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_qqq_moe(2, a, g), "b2q_qqq_moe_down");
+}
+
 // ---- FP8 (e4m3fn, W8A16) layers on the 8-bit tiers ----
 static int fp8_check(const char* fn, const void* packed, const void* scales, const void* out, int K, int N,
                      int group_size, int dtype) {
@@ -536,6 +621,70 @@ int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, in
   DeviceGuard dg(packed);
   return check_cuda(launch_fp8_dequant(packed, scales, out, K, N, group_size, dtype, (cudaStream_t)stream),
                     "b2q_fp8_dequant");
+}
+
+// ---- FP8 MoE experts: the grouped modes of the small-batch tier with the FP8 dequantisation ----
+static int fp8_moe_check(const char* fn, const void* x, const void* packed, const void* scales, const void* out,
+                         const int32_t* counts, const int32_t* offsets, int E, int rows, int K, int N, int group_size,
+                         int dtype) {
+  if (int e = fp8_check(fn, packed, scales, out, K, N, group_size, dtype)) return e;
+  if (x == nullptr || counts == nullptr || offsets == nullptr || !aligned16(x)) {
+    set_error("%s: x, counts and offsets must be device pointers, x 16-byte aligned", fn);
+    return -2;
+  }
+  if (E < 1 || E > 256 || rows < 1) {
+    set_error("%s: E=%d (1..256), rows=%d (>= 1) outside the envelope", fn, E, rows);
+    return -2;
+  }
+  return 0;
+}
+
+int b2q_fp8_moe_gate_up(const void* xs, const void* packed1, const void* scales1, const void* packed3,
+                        const void* scales3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                        int active, int K, int N, int group_size, int dtype, void* stream) {
+  if (int e = fp8_moe_check("b2q_fp8_moe_gate_up", xs, packed1, scales1, h, counts, offsets, E, rows, K, N, group_size,
+                            dtype))
+    return e;
+  if (int e = fp8_check("b2q_fp8_moe_gate_up", packed3, scales3, h, K, N, group_size, dtype)) return e;
+  DeviceGuard dg(packed1);
+  MmArgs a = make_args(xs, packed1, scales1, nullptr, nullptr, nullptr, h, rows, K, N, 8, group_size, dtype, nullptr, 0,
+                       stream);
+  a.fp8 = 1;
+  MoeGroupedArgs g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.packed3 = packed3;
+  g.scales3 = scales3;
+  g.E = E;
+  g.rows = rows;
+  g.active = active;
+  return check_cuda(launch_midm_grouped(1, a, g), "b2q_fp8_moe_gate_up");
+}
+
+int b2q_fp8_moe_down(const void* h, const void* packed2, const void* scales2, const int32_t* counts,
+                     const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair, int E,
+                     int rows, int active, int K, int N, int group_size, int dtype, void* stream) {
+  if (int e = fp8_moe_check("b2q_fp8_moe_down", h, packed2, scales2, ypair, counts, offsets, E, rows, K, N, group_size,
+                            dtype))
+    return e;
+  if (sorted_pairs == nullptr || pair_weights == nullptr) {
+    set_error("b2q_fp8_moe_down: sorted_pairs and pair_weights must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(packed2);
+  MmArgs a = make_args(h, packed2, scales2, nullptr, nullptr, nullptr, ypair, rows, K, N, 8, group_size, dtype, nullptr, 0,
+                       stream);
+  a.fp8 = 1;
+  MoeGroupedArgs g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.sorted_pairs = sorted_pairs;
+  g.pair_weights = pair_weights;
+  g.ypair = ypair;
+  g.E = E;
+  g.rows = rows;
+  g.active = active;
+  return check_cuda(launch_midm_grouped(2, a, g), "b2q_fp8_moe_down");
 }
 
 // ---- block-FP8 (HF / DeepSeek-native, W8A8) tier ----

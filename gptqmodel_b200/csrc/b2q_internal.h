@@ -64,6 +64,22 @@ struct QqqArgs {
 int launch_qqq_quant(const void* x, void* q, float* s_tok, int M, int K, int dtype, cudaStream_t stream);
 int launch_qqq_prepack(const uint8_t* codes, void* packed, int K, int N, int grouped, cudaStream_t stream);
 int launch_qqq_gemm(const QqqArgs& a);
+// grouped (MoE) launches of the QQQ GEMM: a = {q / s_tok = the expert-sorted rows [M = rows, Kp] / [rows], packed /
+// s_channel / s_group = the stacked w1 (mode 1) or w2 (mode 2), out = h [rows, N] (mode 1), N / K of ONE expert}
+struct QqqMoe {
+  const int32_t* counts;        // [E]
+  const int32_t* offsets;       // [E]
+  const int32_t* sorted_pairs;  // [rows]     (mode 2)
+  const float* pair_weights;    // [rows]     (mode 2)
+  const void* packed3;          // mode 1: the up stack, shaped like the gate stack
+  const float* s_channel3;
+  const void* s_group3;
+  float* ypair;                 // mode 2: [rows, N] fp32
+  int E, active;                // experts, experts expected to be active (grid sizing only)
+};
+int launch_qqq_moe(int mode, const QqqArgs& a, const QqqMoe& g);
+int launch_qqq_moe_gather(const void* x, const int32_t* sorted_pairs, void* q, float* s_tok, int rows, int top_k, int K,
+                          int dtype, cudaStream_t stream);
 // block-FP8 (W8A8) tier (b2q_fp8blk.cu)
 struct Fp8BlkArgs {
   const void* x;          // fused decode (M <= 8): the activations [M, K]; else nullptr

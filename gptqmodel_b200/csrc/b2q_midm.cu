@@ -492,7 +492,7 @@ int launch_midm(const MmArgs& a, const void* x) {
 // width hint (largest row count one expert is expected to get), N / K of ONE expert}
 int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
   if ((a.bits != 4 && a.bits != 8) || a.K % MM_BK != 0 || a.N % 32 != 0 || (mode != 1 && mode != 2) || g.E < 1 ||
-      g.rows < 1) {
+      g.rows < 1 || (a.fp8 && (a.bits != 8 || a.qzeros != nullptr))) {
     set_error("b2q_moe: grouped launch needs bits 4 or 8, K %% 64 == 0, N %% 32 == 0 (bits=%d K=%d N=%d E=%d rows=%d)",
               a.bits, a.K, a.N, g.E, g.rows);
     return -1;
@@ -519,10 +519,20 @@ int launch_midm_grouped(int mode, const MmArgs& a, const MoeGroupedArgs& g) {
 #define B2Q_MG_CASE(T)                                                                       \
   (mode == 1 ? (asym ? B2Q_MG_NTOK(T, true, 1) : B2Q_MG_NTOK(T, false, 1))                   \
              : (asym ? B2Q_MG_NTOK(T, true, 2) : B2Q_MG_NTOK(T, false, 2)))
+  // FP8 experts: the ring depths of the 8-bit experts, no zero-points, the e4m3 / scale division in the dequant warps
+#define B2Q_MG_FP8(T, MODE)                                                                                    \
+  (p.ntok == 16   ? launch_midm_t<T, 8, false, 16, 8, 8, MODE, MM_DQG, true>(a, a.x, p, G, grid_z)            \
+   : p.ntok == 32 ? launch_midm_t<T, 8, false, 32, 8, 8, MODE, MM_DQG, true>(a, a.x, p, G, grid_z)            \
+   : p.ntok == 64 ? launch_midm_t<T, 8, false, 64, 4, 8, MODE, MM_DQG, true>(a, a.x, p, G, grid_z)            \
+                  : launch_midm_t<T, 8, false, (MODE == 1 ? 64 : 128), 4, 8, MODE, MM_DQG, true>(a, a.x, p, G, grid_z))
+#define B2Q_MG_FP8_CASE(T) (mode == 1 ? B2Q_MG_FP8(T, 1) : B2Q_MG_FP8(T, 2))
   return launch_split_z((long long)g.E * p.tblocks, [&](int z0, int grid_z) {
     G.route.z0 = z0;
+    if (a.fp8) return a.dtype == 0 ? B2Q_MG_FP8_CASE(__half) : B2Q_MG_FP8_CASE(__nv_bfloat16);
     return a.dtype == 0 ? B2Q_MG_CASE(__half) : B2Q_MG_CASE(__nv_bfloat16);
   });
+#undef B2Q_MG_FP8_CASE
+#undef B2Q_MG_FP8
 #undef B2Q_MG_CASE
 #undef B2Q_MG_NTOK
 #undef B2Q_MG_NTOK8

@@ -10,6 +10,11 @@
 //     block (one feature row per thread) into int8 rows; warps 0..3 issue m64nNk32.s32.s8.s8 into int32 registers.  The
 //     `ks` CTAs of a cluster split the k-blocks of a tile and reduce their integer partials over distributed shared
 //     memory, so any split gives the same bits; token blocks of NTOK rows are spread over gridDim.z.  No atomics.
+//   * qqq_moe_gemm_kernel: grouped modes of the same GEMM body for MoE experts (MODE 1 / 2) over the expert-sorted rows
+//     of b2q_moe_align, the weights the stacks of all experts.  MODE 1 pairs 64 gate features (w1, m64 block 0) with
+//     the same 64 up features (w3, m64 block 1) in one 128-row tile and stores h = T(T(silu(g)) * u); MODE 2 (down)
+//     stores w[pair] * T(y) in fp32 to the pair's row of ypair.
+//   * qqq_moe_gather_kernel: the quantiser over the sorted rows, row i quantising token sorted_pairs[i] / top_k.
 //
 // Packed weights (b2q_qqq_prepack): tile (nt, kb) of 128 features x 128 k is 8 KB at ((nt * KB + kb) * 8192), laid out
 // uint4 [4 quads][128 features]: quad q of feature f holds k = 32 q .. 32 q + 31 as four 32-bit words of eight nibbles.
@@ -71,14 +76,12 @@ __device__ __forceinline__ int quant_code(float a, float s) {
   return (int)fminf(fmaxf(rintf(v), -128.f), 127.f);
 }
 
+// one CTA quantises one row: token `xrow` of x [*, K] -> codes row `row` of q [*, Kp] and s_tok[row]
 template <typename T>
-__global__ void __launch_bounds__(Q_QUANT_THREADS)
-    qqq_quant_kernel(const T* __restrict__ x, int8_t* __restrict__ q, float* __restrict__ s_tok, int K, int Kp) {
+__device__ __forceinline__ void qqq_quant_row(const T* __restrict__ x, int8_t* __restrict__ q, float* __restrict__ s_tok,
+                                              int K, int Kp, int xrow, int row) {
   __shared__ float red[Q_QUANT_THREADS / 32];
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");  // x is the previous kernel's output
-  const int row = blockIdx.x;
-  const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * K);
+  const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)xrow * K);
   const int n8 = K >> 3;
   float amax = 0.f;
   for (int i = threadIdx.x; i < n8; i += Q_QUANT_THREADS) {
@@ -113,6 +116,27 @@ __global__ void __launch_bounds__(Q_QUANT_THREADS)
     }
     qr[i] = make_uint2(w[0], w[1]);
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(Q_QUANT_THREADS)
+    qqq_quant_kernel(const T* __restrict__ x, int8_t* __restrict__ q, float* __restrict__ s_tok, int K, int Kp) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // x is the previous kernel's output
+  const int row = blockIdx.x;
+  qqq_quant_row<T>(x, q, s_tok, K, Kp, row, row);
+}
+
+// the quantiser over the expert-sorted rows of a MoE block: row i is token sorted_pairs[i] / top_k of x [T, K], so its
+// codes and scale are those qqq_quant_kernel gives that token
+template <typename T>
+__global__ void __launch_bounds__(Q_QUANT_THREADS)
+    qqq_moe_gather_kernel(const T* __restrict__ x, const int32_t* __restrict__ sorted_pairs, int8_t* __restrict__ q,
+                          float* __restrict__ s_tok, int top_k, int K, int Kp) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // sorted_pairs (and x) are the previous kernels' output
+  const int row = blockIdx.x;
+  qqq_quant_row<T>(x, q, s_tok, K, Kp, sorted_pairs[row] / top_k, row);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -165,12 +189,24 @@ __device__ __forceinline__ void expand_group(uint32_t w, uint32_t s2, uint32_t& 
   hi = __byte_perm(h[2], h[3], 0x6240);
 }
 
-template <int NTOK, bool GROUPED>
-__global__ void __launch_bounds__(Q_THREADS, 1)
-    qqq_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const uint4* __restrict__ packed,
-                    const float* __restrict__ s_channel, const __half* __restrict__ s_group,
-                    const float* __restrict__ s_tok, const __half* __restrict__ bias, void* __restrict__ out, int M,
-                    int KB, int N, int kpc, int out_bf16) {
+// grouped launches (MODE 1 / 2) over the experts of a MoE block: the stacks hold E experts back to back, one expert's
+// b2q_qqq_packed_bytes(K, N), N channel scales and K/128 x N group scales apart
+struct QqqMoeArgs {
+  MoeRoute route;
+  const uint4* packed3;     // MODE 1: the w3 (up) stack, shaped like the w1 (gate) stack
+  const float* s_channel3;
+  const __half* s_group3;
+};
+
+// the GEMM of qqq_gemm_kernel (MODE 0) and qqq_moe_gemm_kernel (MODE 1 / 2, G their grouped arguments).  MODE 1 pairs 64
+// gate features (w1, m64 block 0) with the same 64 up features (w3, m64 block 1) in one 128-row tile and stores
+// h = T(T(silu(g)) * u); MODE 2 (down) stores w[pair] * T(y) in fp32 to the pair's row of ypair
+template <int NTOK, bool GROUPED, int MODE>
+__device__ __forceinline__ void qqq_gemm_body(const CUtensorMap& tmap_q, const uint4* __restrict__ packed,
+                                              const float* __restrict__ s_channel, const __half* __restrict__ s_group,
+                                              const float* __restrict__ s_tok, const __half* __restrict__ bias,
+                                              void* __restrict__ out, int M, int KB, int N, int kpc, int out_bf16,
+                                              const QqqMoeArgs* G) {
   using C = QqqCfg<NTOK>;
   constexpr int PST = C::PST, WST = C::WST, XST = C::XST;
   extern __shared__ uint8_t smem_raw[];
@@ -184,8 +220,25 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
   const uint32_t bar_wready = bar_xempty + 8 * XST, bar_wempty = bar_wready + 8 * WST;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nt = blockIdx.x, n0 = nt * Q_BF;
-  const int row0 = blockIdx.z * NTOK;
+  const int nt = blockIdx.x, n0 = nt * (MODE == 1 ? Q_BF / 2 : Q_BF);  // MODE 1: 64 gate + 64 up features
+  int row0 = blockIdx.z * NTOK, rows = NTOK;  // first row and row bound of this CTA's token block
+  const uint4* packed3 = nullptr;
+  const float* s_channel3 = nullptr;
+  const __half* s_group3 = nullptr;
+  if (MODE != 0) {
+    int e;
+    if (!moe_block<NTOK>(G->route, e, row0, rows)) return;
+    // one expert: KB x ceil(N/128) packed tiles, N channel scales, KB x N group scales
+    const size_t pstride = (size_t)KB * ((N + Q_BF - 1) / Q_BF) * (Q_TILE_BYTES / 16);
+    packed += (size_t)e * pstride;
+    s_channel += (size_t)e * N;
+    if (GROUPED) s_group += (size_t)e * KB * N;
+    if (MODE == 1) {
+      packed3 = G->packed3 + (size_t)e * pstride;
+      s_channel3 = G->s_channel3 + (size_t)e * N;
+      if (GROUPED) s_group3 = G->s_group3 + (size_t)e * KB * N;
+    }
+  }
   const uint32_t nrank = cluster_nctarank(), crank = cluster_ctarank();
   const int kb0 = (int)crank * kpc, kb1 = min(KB, kb0 + kpc);
   const int nkb = kb1 - kb0;
@@ -207,10 +260,25 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
   }
   __syncthreads();
 
-  const uint4* ptile = packed + (size_t)nt * KB * (Q_TILE_BYTES / 16);
+  // MODE 1: the tile's 64 gate and 64 up features are one half of packed tile n0 / 128 of each stack
+  const uint4* ptile = packed + (size_t)(MODE == 1 ? n0 / Q_BF : nt) * KB * (Q_TILE_BYTES / 16);
+  const uint4* ptile3 = MODE == 1 ? packed3 + (size_t)(n0 / Q_BF) * KB * (Q_TILE_BYTES / 16) : nullptr;
   auto load_weights = [&](int i, int s) {
     mbar_expect_tx(bar_pfull + 8 * s, Q_TILE_BYTES);
-    bulk_load(sP + s * Q_TILE_BYTES, ptile + (size_t)(kb0 + i) * (Q_TILE_BYTES / 16), Q_TILE_BYTES, bar_pfull + 8 * s);
+    if (MODE == 1) {
+      // quad q of a packed tile is [128 features] x 16 bytes: the 64-feature half of each stack is one 1 KB run per
+      // quad, staged as features 0..63 (gate) and 64..127 (up) of the stage's quad
+      const int half = (n0 / (Q_BF / 2)) & 1;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const size_t src = (size_t)(kb0 + i) * (Q_TILE_BYTES / 16) + q * Q_BF + half * (Q_BF / 2);
+        const uint32_t dst = sP + s * Q_TILE_BYTES + q * Q_BF * 16;
+        bulk_load(dst, ptile + src, Q_TILE_BYTES / 8, bar_pfull + 8 * s);
+        bulk_load(dst + Q_TILE_BYTES / 8, ptile3 + src, Q_TILE_BYTES / 8, bar_pfull + 8 * s);
+      }
+    } else {
+      bulk_load(sP + s * Q_TILE_BYTES, ptile + (size_t)(kb0 + i) * (Q_TILE_BYTES / 16), Q_TILE_BYTES, bar_pfull + 8 * s);
+    }
   };
 
   if (warp == 8) {
@@ -260,7 +328,9 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
   } else {
     // ================================ dequant warps ================================
     const int f = threadIdx.x - Q_MMA_THREADS;  // feature row of the tile
-    const int n = n0 + f;
+    // MODE 1: rows 0..63 expand gate feature n0 + f of w1, rows 64..127 up feature n0 + f - 64 of w3
+    const int n = MODE == 1 ? n0 + (f & (Q_BF / 2 - 1)) : n0 + f;
+    const __half* sgr = (MODE == 1 && f >= Q_BF / 2) ? s_group3 : s_group;
     // the weight stream of the first PST blocks starts at once (under programmatic dependent launch: while the
     // quantiser still runs)
     if (f == 0)
@@ -269,7 +339,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
       const int s = i % PST, ws = i % WST;
       uint32_t s2 = 0;
       if (GROUPED) {
-        const __half sg = n < N ? s_group[(size_t)(kb0 + i) * N + n] : __float2half_rn(0.f);
+        const __half sg = n < N ? sgr[(size_t)(kb0 + i) * N + n] : __float2half_rn(0.f);
         const __half2 sg2 = __halves2half2(sg, sg);
         s2 = *reinterpret_cast<const uint32_t*>(&sg2);
       }
@@ -306,13 +376,38 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
   asm volatile("griddepcontrol.wait;" ::: "memory");  // (already satisfied) orders the global stores below
   __syncwarp();
   cluster_sync_all();
-  if (warp < Q_RED_WARPS) {
+  // the reference epilogue: fp32(acc) * s_channel * s_tok, rounded to fp16
+  auto y16 = [](int a, float sc, float st) { return __float2half_rn(__fmul_rn(__fmul_rn(__int2float_rn(a), sc), st)); };
+  if (MODE == 1 && warp < Q_RED_WARPS) {
+    // rank z reduces token rows z, z + nrank, ... , a half-warp per row: lane l holds gate features 4 (l & 15) .. + 3 of
+    // the tile (those columns of h) and their up features at + 64
+    const int hw = 2 * warp + (lane >> 4), c = lane & 15;
+    const int nc = n0 + 4 * c;
+    const float4 sg4 = *reinterpret_cast<const float4*>(s_channel + nc);
+    const float4 su4 = *reinterpret_cast<const float4*>(s_channel3 + nc);
+    const float scg[4] = {sg4.x, sg4.y, sg4.z, sg4.w}, scu[4] = {su4.x, su4.y, su4.z, su4.w};
+    for (int tok = (int)crank + (int)nrank * hw; tok < rows; tok += (int)nrank * (2 * Q_RED_WARPS)) {
+      int a[2][4];
+      dsmem_sum4<2, true>(sW + (uint32_t)tok * (Q_BF * 4) + (uint32_t)c * 16, (Q_BF / 2) * 4, nrank, a);
+      const float st = s_tok[row0 + tok];
+      float g[4], u[4];  // the fp16 values of the layers' outputs
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        g[e] = __half2float(y16(a[0][e], scg[e], st));
+        u[e] = __half2float(y16(a[1][e], scu[e], st));
+      }
+      const size_t o = (size_t)(row0 + tok) * N + nc;
+      if (out_bf16) store_silu_mul4(reinterpret_cast<__nv_bfloat16*>(out) + o, g, u);
+      else store_silu_mul4(reinterpret_cast<__half*>(out) + o, g, u);
+    }
+  } else if (MODE != 1 && warp < Q_RED_WARPS) {
     // rank z reduces token rows z, z + nrank, ... over all ranks: integer sums, so the order does not matter
     const int chunk = threadIdx.x & 31;
     const int nc = n0 + chunk * 4;
     if (nc < N) {
       const float4 sc = *reinterpret_cast<const float4*>(s_channel + nc);
-      for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && row0 + tok < M; tok += (int)nrank * Q_RED_WARPS) {
+      for (int tok = (int)crank + (int)nrank * warp; tok < NTOK && tok < rows && row0 + tok < M;
+           tok += (int)nrank * Q_RED_WARPS) {
         int a[1][4];
         dsmem_sum4<1, true>(sW + (uint32_t)tok * (Q_BF * 4) + (uint32_t)chunk * 16, 0, nrank, a);
         const int m = row0 + tok;
@@ -321,11 +416,17 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
         __half y[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          // the reference epilogue: fp32(acc) * s_channel * s_tok, rounded to fp16; then D.add_(bias)
-          y[e] = __float2half_rn(__fmul_rn(__fmul_rn(__int2float_rn(a[0][e]), scs[e]), st));
+          // then D.add_(bias)
+          y[e] = y16(a[0][e], scs[e], st);
           if (bias != nullptr) y[e] = __float2half_rn(__half2float(y[e]) + __half2float(bias[nc + e]));
         }
-        if (out_bf16) {
+        if (MODE == 2) {
+          const int pair = G->route.sorted_pairs[m];
+          float* yp = G->route.ypair + (size_t)pair * N + nc;
+          const float yf[4] = {__half2float(y[0]), __half2float(y[1]), __half2float(y[2]), __half2float(y[3])};
+          if (out_bf16) store_ypair4<__nv_bfloat16>(yp, G->route.pair_weights[pair], yf);
+          else store_ypair4<__half>(yp, G->route.pair_weights[pair], yf);
+        } else if (out_bf16) {
           __nv_bfloat16 b[4];
 #pragma unroll
           for (int e = 0; e < 4; ++e) b[e] = __float2bfloat16_rn(__half2float(y[e]));
@@ -340,6 +441,28 @@ __global__ void __launch_bounds__(Q_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
+}
+
+template <int NTOK, bool GROUPED>
+__global__ void __launch_bounds__(Q_THREADS, 1)
+    qqq_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const uint4* __restrict__ packed,
+                    const float* __restrict__ s_channel, const __half* __restrict__ s_group,
+                    const float* __restrict__ s_tok, const __half* __restrict__ bias, void* __restrict__ out, int M,
+                    int KB, int N, int kpc, int out_bf16) {
+  qqq_gemm_body<NTOK, GROUPED, 0>(tmap_q, packed, s_channel, s_group, s_tok, bias, out, M, KB, N, kpc, out_bf16,
+                                  nullptr);
+}
+
+// grouped launches over the experts of a MoE block: M = rows, N / K of one expert, out = h (MODE 1); the stacks of w1
+// (MODE 1) or w2 (MODE 2) in packed / s_channel / s_group
+template <int NTOK, bool GROUPED, int MODE>
+__global__ void __launch_bounds__(Q_THREADS, 1)
+    qqq_moe_gemm_kernel(const __grid_constant__ CUtensorMap tmap_q, const uint4* __restrict__ packed,
+                        const float* __restrict__ s_channel, const __half* __restrict__ s_group,
+                        const float* __restrict__ s_tok, void* __restrict__ out, int M, int KB, int N, int kpc,
+                        int out_bf16, const __grid_constant__ QqqMoeArgs G) {
+  qqq_gemm_body<NTOK, GROUPED, MODE>(tmap_q, packed, s_channel, s_group, s_tok, nullptr, out, M, KB, N, kpc, out_bf16,
+                                     &G);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -400,6 +523,70 @@ int launch_qqq_gemm(const QqqArgs& a) {
     case 64: return g ? launch_qqq_gemm_t<64, true>(a, p) : launch_qqq_gemm_t<64, false>(a, p);
     default: return g ? launch_qqq_gemm_t<128, true>(a, p) : launch_qqq_gemm_t<128, false>(a, p);
   }
+}
+
+int launch_qqq_moe_gather(const void* x, const int32_t* sorted_pairs, void* q, float* s_tok, int rows, int top_k, int K,
+                          int dtype, cudaStream_t stream) {
+  const int Kp = (K + Q_BK - 1) / Q_BK * Q_BK;
+  if (dtype == 0)
+    return launch_kernel(qqq_moe_gather_kernel<__half>, dim3(rows, 1, 1), dim3(Q_QUANT_THREADS, 1, 1), 0, stream, 0,
+                         true, (const __half*)x, sorted_pairs, (int8_t*)q, s_tok, top_k, K, Kp);
+  return launch_kernel(qqq_moe_gather_kernel<__nv_bfloat16>, dim3(rows, 1, 1), dim3(Q_QUANT_THREADS, 1, 1), 0, stream, 0,
+                       true, (const __nv_bfloat16*)x, sorted_pairs, (int8_t*)q, s_tok, top_k, K, Kp);
+}
+
+// grouped launches: the token box of qqq_plan for all rows; split-K ranks fill the SMs with the CTAs of all rows' token
+// blocks or of `active` experts' first blocks, whichever is more (the rule of fp8blk_plan)
+static SwapPlan qqq_moe_plan(int mode, int M, int K, int N, int active) {
+  const int KB = (K + Q_BK - 1) / Q_BK, fb = mode == 1 ? Q_BF / 2 : Q_BF, tiles = (N + fb - 1) / fb;
+  SwapPlan p;
+  p.ntok = swap_ntok(M, 8, 128);
+  p.tblocks = (M + p.ntok - 1) / p.ntok;
+  if (active < 1) active = 1;
+  p.ks = trim_ranks(split_k_ranks((long long)tiles * (p.tblocks > active ? p.tblocks : active), KB, 2), KB);
+  p.kpc = (KB + p.ks - 1) / p.ks;
+  return p;
+}
+
+template <int NTOK, bool GROUPED, int MODE>
+static int launch_qqq_moe_t(const QqqArgs& a, const QqqMoe& g, const SwapPlan& p) {
+  using C = QqqCfg<NTOK>;
+  const int KB = (a.K + Q_BK - 1) / Q_BK;
+  CUtensorMap tmap;  // the sorted rows' codes [M, Kp]; a box may run into the next expert's rows, which are not stored
+  if (make_tmap_2d(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.q, KB * Q_BK, a.M, (size_t)KB * Q_BK, Q_BK, NTOK,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  QqqMoeArgs G = {};
+  G.route = {g.counts, g.offsets, g.sorted_pairs, g.pair_weights, g.ypair, p.tblocks, 0};
+  G.packed3 = (const uint4*)g.packed3;
+  G.s_channel3 = g.s_channel3;
+  G.s_group3 = (const __half*)g.s_group3;
+  auto kern = qqq_moe_gemm_kernel<NTOK, GROUPED, MODE>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_qqq_moe")) return e;
+  const int tiles = (a.N + (MODE == 1 ? Q_BF / 2 : Q_BF) - 1) / (MODE == 1 ? Q_BF / 2 : Q_BF);
+  return launch_split_z((long long)g.E * p.tblocks, [&](int z0, int grid_z) {
+    G.route.z0 = z0;
+    return launch_kernel(kern, dim3(tiles, p.ks, grid_z), dim3(Q_THREADS, 1, 1), C::SMEM_BYTES, a.stream, p.ks, true,
+                         tmap, (const uint4*)a.packed, a.s_channel, (const __half*)a.s_group, a.s_tok, a.out, a.M, KB,
+                         a.N, p.kpc, a.out_dtype, G);
+  });
+}
+
+int launch_qqq_moe(int mode, const QqqArgs& a, const QqqMoe& g) {
+  const bool gr = a.s_group != nullptr;
+  const SwapPlan p = qqq_moe_plan(mode, a.M, a.K, a.N, g.active);
+#define B2Q_QQM(NTOK) \
+  return mode == 1 ? (gr ? launch_qqq_moe_t<NTOK, true, 1>(a, g, p) : launch_qqq_moe_t<NTOK, false, 1>(a, g, p)) \
+                   : (gr ? launch_qqq_moe_t<NTOK, true, 2>(a, g, p) : launch_qqq_moe_t<NTOK, false, 2>(a, g, p));
+  switch (p.ntok) {
+    case 8: B2Q_QQM(8)
+    case 16: B2Q_QQM(16)
+    case 32: B2Q_QQM(32)
+    case 64: B2Q_QQM(64)
+    default: B2Q_QQM(128)
+  }
+#undef B2Q_QQM
 }
 
 }  // namespace b2q

@@ -23,6 +23,12 @@ per-expert loop, arranged for the B200 kernels and for tensor parallelism:
     gate|up launch, the quantiser on h, ONE grouped down launch, combine (grouped modes of b2q_fp8blk.cu; include/b2q.h
     states the rounding points, those of transformers' per-expert FP8Linear loop).  The checkpoint tensors are stacked
     once and the modules keep views into the stack;
+  * QQQ experts (every w1 / w3 / w2 a post_init'ed B200QqqQuantLinear, W4A8): the same six launches on the int8 tensor
+    cores — align, gather-and-quantise, ONE grouped gate|up launch, the quantiser on h, ONE grouped down launch, combine
+    (grouped modes of b2q_qqq.cu; include/b2q.h states the rounding points, those of the per-expert QQQLinear loop);
+  * FP8 W8A16 experts (every w1 / w3 / w2 a post_init'ed B200Fp8QuantLinear): the five launches of the GPTQ grouped path
+    on the FP8 instantiations of the grouped small-batch kernels, W the exact b2q_fp8_dequant operand.  Both keep the
+    modules working on views into the stacks;
   * LOOP path (fallback: dense stand-ins in CPU tests, mixed experts, regrouped act-order shards): tokens are sorted by
     expert once, every expert sees one contiguous block of its routed tokens; one host sync per block for the per-expert
     counts, like the reference's loop;
@@ -76,7 +82,11 @@ class MoEExperts(torch.nn.Module):
                                  "group size, with one kernel bit width (4 or 8) for w1 / w3 and one for w2, the same "
                                  "act-order permutation in w1 and w3 of every expert, and no regrouped g_idx, bias or "
                                  "adapters; or post_init'ed B200BlockFp8Linears only, one shape per role on one device, "
-                                 "an intermediate size that is a multiple of 128, and no bias or adapters")
+                                 "an intermediate size that is a multiple of 128, and no bias or adapters; or post_init'ed "
+                                 "B200QqqQuantLinears only (one shape and group kind per role, w1 and w3 alike, an "
+                                 "intermediate size that is a multiple of 64, at most 256 experts on one device, no bias "
+                                 "or adapters); or post_init'ed B200Fp8QuantLinears only (one shape and scale group per "
+                                 "role, at most 256 experts on one device, no bias or adapters)")
         if fuse and self._stack is None:
             from .qlinear import B200KernelMixin, fuse_siblings
 
@@ -89,8 +99,16 @@ class MoEExperts(torch.nn.Module):
         from .fp8_block import B200BlockFp8Linear
         from .qlinear import B200KernelMixin
 
-        if all(isinstance(m, B200BlockFp8Linear) for mods in (self.w1, self.w3, self.w2) for m in mods):
+        from .fp8 import B200Fp8QuantLinear
+        from .qqq import B200QqqQuantLinear
+
+        every = [m for mods in (self.w1, self.w3, self.w2) for m in mods]
+        if all(isinstance(m, B200BlockFp8Linear) for m in every):
             return self._build_fp8blk_stack()
+        if all(isinstance(m, B200QqqQuantLinear) for m in every):
+            return self._build_qqq_stack()
+        if all(isinstance(m, B200Fp8QuantLinear) for m in every):
+            return self._build_fp8_stack()
         sets = []
         for mods in (self.w1, self.w3, self.w2):
             m0 = mods[0]
@@ -164,6 +182,144 @@ class MoEExperts(torch.nn.Module):
                     m.weight_scale_inv = scale[e]
             out[name] = dict(weight=weight, scale=scale, K=mods[0].in_features, N=mods[0].out_features)
         return out
+
+    def _role_ok(self, attrs):
+        """The checks every role of a QQQ / FP8 stack passes: post_init'ed, no bias or adapter, one value of `attrs` per
+        role, w1 and w3 alike, w2 reading the intermediate size, at most 256 experts."""
+        w1, w3, w2 = list(self.w1), list(self.w3), list(self.w2)
+        if len(w1) > 256:
+            return False
+        for mods in (w1, w3, w2):
+            for m in mods:
+                if not m._prepacked or m.bias is not None or m.adapter or attrs(m) != attrs(mods[0]):
+                    return False
+        return attrs(w1[0]) == attrs(w3[0]) and w2[0].in_features == w1[0].out_features
+
+    def _build_qqq_stack(self):
+        """Stack the QQQ experts' prepacked tensors (packed [E, bytes], s_channel [E, N], s_group [E, K/128, N]) for the
+        grouped int8 kernels; None if the experts do not qualify."""
+        if not self._role_ok(lambda m: (m.in_features, m.out_features, m._kgs, m.packed.device)):
+            return None
+        if self.w1[0].out_features % 64 != 0:  # gate|up tiles pair 64 gate with 64 up features
+            return None
+        out = {"qqq": True}
+        for name, mods in (("w1", self.w1), ("w3", self.w3), ("w2", self.w2)):
+            packed = torch.stack([m.packed for m in mods]).contiguous()
+            sc = torch.stack([m._sc for m in mods]).contiguous()
+            sg = torch.stack([m._sg for m in mods]).contiguous() if mods[0]._kgs == 128 else None
+            for e, m in enumerate(mods):  # the modules keep working on their own; no second copy of the weights
+                m.packed, m._sc = packed[e], sc[e]
+                if sg is not None:
+                    m._sg = sg[e]
+            out[name] = dict(packed=packed, sc=sc, sg=sg, K=mods[0].in_features, N=mods[0].out_features,
+                             group=mods[0]._kgs)
+        return out
+
+    def _build_fp8_stack(self):
+        """Stack the FP8 (W8A16) experts' prepacked codes and per-dtype scale tables [E, K/g, N] for the grouped
+        small-batch kernels; None if the experts do not qualify."""
+        if not self._role_ok(lambda m: (m.in_features, m.out_features, m._gs, m.packed.device)):
+            return None
+        out = {"fp8": True}
+        for name, mods in (("w1", self.w1), ("w3", self.w3), ("w2", self.w2)):
+            packed = torch.stack([m.packed for m in mods]).contiguous()
+            scales = {dt: torch.stack([m._scales[dt] for m in mods]).contiguous() for dt in mods[0]._scales}
+            for e, m in enumerate(mods):  # the modules keep working on their own; no second copy of the weights
+                m.packed = packed[e]
+                for dt, st in scales.items():
+                    m._scales[dt] = st[e]
+            out[name] = dict(packed=packed, scales=scales, K=mods[0].in_features, N=mods[0].out_features,
+                             group=mods[0]._gs, fp16_ok=all(m._fp16_ok for m in mods))
+        return out
+
+    def _check_x(self, x, T, top_k, K, topk_weights, dev):
+        # the gather kernels read x [T, K] by token index: a mismatched x would be read out of bounds
+        if x.dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError(f"MoEExperts: quantised experts take fp16 / bf16 activations, got {x.dtype}")
+        if tuple(x.shape) != (T, K) or x.device != dev or tuple(topk_weights.shape) != (T, top_k):
+            raise ValueError(f"MoEExperts: x {tuple(x.shape)} on {x.device} does not fit [{T}, {K}] on {dev}, "
+                             f"or topk_weights {tuple(topk_weights.shape)} is not [{T}, {top_k}]")
+
+    def _forward_grouped_qqq(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
+        """QQQ experts: align -> gather-and-quantise -> gate|up -> quantise h -> down -> combine (include/b2q.h)."""
+        from ._lib import check, lib
+
+        T, top_k = topk_ids.shape
+        rows, E = T * top_k, self.num_experts
+        s1, s3, s2 = self._stack["w1"], self._stack["w3"], self._stack["w2"]
+        K, inter, Kout = s1["K"], s1["N"], s2["N"]
+        self._check_x(x, T, top_k, K, topk_weights, s1["packed"].device)
+        dev, dt = x.device, x.dtype
+        code = 0 if dt == torch.float16 else 1
+        st = torch.cuda.current_stream(dev).cuda_stream
+        ids = topk_ids.to(torch.int32).contiguous()
+        wts = topk_weights.to(torch.float32).contiguous()
+        x2 = x.contiguous()
+        if x2.data_ptr() % 16 != 0:
+            x2 = x2.clone()
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        kp = lambda k: (k + 127) // 128 * 128  # noqa: E731  (codes rows are padded to 128 k)
+        tables = torch.empty(2 * E + rows, dtype=torch.int32, device=dev)
+        counts, offsets, sorted_pairs = tables[:E], tables[E:2 * E], tables[2 * E:]
+        codes = torch.empty((rows, kp(K)), dtype=torch.int8, device=dev)
+        s_x = torch.empty(rows, dtype=torch.float32, device=dev)
+        h = torch.empty((rows, inter), dtype=dt, device=dev)
+        codes_h = torch.empty((rows, kp(inter)), dtype=torch.int8, device=dev)
+        s_h = torch.empty(rows, dtype=torch.float32, device=dev)
+        ypair = torch.empty((rows, Kout), dtype=torch.float32, device=dev)
+        y = torch.empty((T, Kout), dtype=dt, device=dev)
+        active = min(E, rows)
+        check(lib.b2q_moe_align(p(ids), T, top_k, E, p(counts), p(offsets), p(sorted_pairs), st), "b2q_moe_align")
+        check(lib.b2q_qqq_moe_gather(p(x2), p(sorted_pairs), p(codes), p(s_x), T, top_k, K, code, st),
+              "b2q_qqq_moe_gather")
+        check(lib.b2q_qqq_moe_gate_up(p(codes), p(s_x), p(s1["packed"]), p(s1["sc"]), p(s1["sg"]), p(s3["packed"]),
+                                      p(s3["sc"]), p(s3["sg"]), p(h), p(counts), p(offsets), E, rows, active, K, inter,
+                                      s1["group"], code, st), "b2q_qqq_moe_gate_up")
+        check(lib.b2q_qqq_quantize(p(h), p(codes_h), p(s_h), rows, inter, code, st), "b2q_qqq_quantize")
+        check(lib.b2q_qqq_moe_down(p(codes_h), p(s_h), p(s2["packed"]), p(s2["sc"]), p(s2["sg"]), p(counts),
+                                   p(offsets), p(sorted_pairs), p(wts), p(ypair), E, rows, active, inter, Kout,
+                                   s2["group"], code, st), "b2q_qqq_moe_down")
+        check(lib.b2q_moe_combine(p(ypair), p(y), T, top_k, Kout, code, st), "b2q_moe_combine")
+        return y
+
+    def _forward_grouped_fp8(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
+        """FP8 (W8A16) experts: align -> gather -> gate|up -> down -> combine on the grouped small-batch kernels."""
+        from ._lib import check, lib
+
+        T, top_k = topk_ids.shape
+        rows, E = T * top_k, self.num_experts
+        s1, s3, s2 = self._stack["w1"], self._stack["w3"], self._stack["w2"]
+        K, inter, Kout = s1["K"], s1["N"], s2["N"]
+        self._check_x(x, T, top_k, K, topk_weights, s1["packed"].device)
+        dev, dt = x.device, x.dtype
+        if dt == torch.float16 and not all(s["fp16_ok"] for s in (s1, s3, s2)):
+            raise ValueError("MoEExperts: a weight_scale_inv of the FP8 experts overflows fp16 (> 65504): fp16 "
+                             "activations would give zero weights; run this block in bf16")
+        code = 0 if dt == torch.float16 else 1
+        st = torch.cuda.current_stream(dev).cuda_stream
+        ids = topk_ids.to(torch.int32).contiguous()
+        wts = topk_weights.to(torch.float32).contiguous()
+        x2 = x.contiguous()
+        if x2.data_ptr() % 16 != 0:
+            x2 = x2.clone()
+        p = lambda t: t.data_ptr()  # noqa: E731
+        tables = torch.empty(2 * E + rows, dtype=torch.int32, device=dev)
+        counts, offsets, sorted_pairs = tables[:E], tables[E:2 * E], tables[2 * E:]
+        xs = torch.empty((rows, K), dtype=dt, device=dev)
+        h = torch.empty((rows, inter), dtype=dt, device=dev)
+        ypair = torch.empty((rows, Kout), dtype=torch.float32, device=dev)
+        y = torch.empty((T, Kout), dtype=dt, device=dev)
+        active = min(E, rows)
+        check(lib.b2q_moe_align(p(ids), T, top_k, E, p(counts), p(offsets), p(sorted_pairs), st), "b2q_moe_align")
+        check(lib.b2q_moe_gather(p(x2), p(sorted_pairs), p(xs), rows, top_k, K, st), "b2q_moe_gather")
+        check(lib.b2q_fp8_moe_gate_up(p(xs), p(s1["packed"]), p(s1["scales"][dt]), p(s3["packed"]),
+                                      p(s3["scales"][dt]), p(h), p(counts), p(offsets), E, rows, active, K, inter,
+                                      s1["group"], code, st), "b2q_fp8_moe_gate_up")
+        check(lib.b2q_fp8_moe_down(p(h), p(s2["packed"]), p(s2["scales"][dt]), p(counts), p(offsets), p(sorted_pairs),
+                                   p(wts), p(ypair), E, rows, active, inter, Kout, s2["group"], code, st),
+              "b2q_fp8_moe_down")
+        check(lib.b2q_moe_combine(p(ypair), p(y), T, top_k, Kout, code, st), "b2q_moe_combine")
+        return y
 
     def _forward_grouped_fp8blk(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
         """Block-FP8 experts: align -> gather-and-quantise -> gate|up -> quantise h -> down -> combine (include/b2q.h)."""
@@ -306,6 +462,10 @@ class MoEExperts(torch.nn.Module):
         if self._stack is not None and x.is_cuda and x.dim() == 2:
             if "fp8blk" in self._stack:
                 out = self._forward_grouped_fp8blk(x, topk_ids, topk_weights)
+            elif "qqq" in self._stack:
+                out = self._forward_grouped_qqq(x, topk_ids, topk_weights)
+            elif "fp8" in self._stack:
+                out = self._forward_grouped_fp8(x, topk_ids, topk_weights)
             else:
                 out = self._forward_grouped(x, topk_ids, topk_weights)
             if self.reduce is not None and out.numel() <= self.reduce.max_elems and out.numel() % 8 == 0:

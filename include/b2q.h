@@ -248,6 +248,36 @@ int b2q_qqq_forward(const void* x, const void* packed, const float* s_channel, c
                     void* out, int M, int K, int N, int group_size, int dtype, int out_dtype, void* workspace,
                     size_t workspace_bytes, void* stream);
 
+/* QQQ MoE experts (an addition to ABI v8): each role's experts stacked back to back — packed [E, b2q_qqq_packed_bytes(K,
+ * N)], s_channel fp32 [E, N], s_group fp16 [E, K/128, N] (NULL exactly for group_size -1) — and the routing tables of
+ * b2q_moe_align.  One block is six launches with no host synchronisation: b2q_moe_align, b2q_qqq_moe_gather,
+ * b2q_qqq_moe_gate_up, b2q_qqq_quantize of h, b2q_qqq_moe_down, b2q_moe_combine.  For every routed pair (token t, slot j,
+ * expert e), with Q the quantiser and F the layer arithmetic of b2q_qqq_mm above (F rounds to fp16):
+ *   (q, s)     = Q(x_t)                           (the codes b2q_qqq_quantize gives the token)
+ *   g = T(F(q, s, W1_e)),  u = T(F(q, s, W3_e))   (for T = bf16: bf16 of the fp16 value, as QQQLinear returns it)
+ *   h = T(T(silu(g)) * u)                         (silu(g) = g / (1 + __expf(-g)) in fp32)
+ *   (q_h, s_h) = Q(h)                             (down_proj quantises its own input; bf16 h goes through fp16 first)
+ *   yp_j = T(F(q_h, s_h, W2_e))
+ *   y_t  = T(sum_j fp32(w_j * yp_j))              (fp32, slot order, one rounding: b2q_moe_combine)
+ * These are the rounding points of the reference model's per-expert loop over QQQLinear modules.  The accumulation is
+ * int32 and exact, so the gate / up values and the down output of each expert's rows equal b2q_qqq_mm on those rows for
+ * any split.  Envelope: each matmul meets the shape envelope of b2q_qqq_mm, the intermediate size N of gate|up is a
+ * multiple of 64, w1 and w3 share one group_size, E <= 256; the pointers as for b2q_qqq_mm. */
+/* q int8 [T*top_k, Kp], s_tok fp32 [T*top_k]: sorted row i = Q(x[sorted_pairs[i] / top_k]) (Kp = K rounded up to 128). */
+int b2q_qqq_moe_gather(const void* x, const int32_t* sorted_pairs, int8_t* q, float* s_tok, int T, int top_k, int K,
+                       int dtype, void* stream);
+/* h T [rows, N] (dtype = T of the block): w1 / w3 stacks of one group_size, N = the intermediate size; active = experts
+ * expected to hold rows (grid sizing). */
+int b2q_qqq_moe_gate_up(const int8_t* q, const float* s_tok, const void* packed1, const float* s_channel1,
+                        const void* s_group1, const void* packed3, const float* s_channel3, const void* s_group3, void* h,
+                        const int32_t* counts, const int32_t* offsets, int E, int rows, int active, int K, int N,
+                        int group_size, int dtype, void* stream);
+/* ypair fp32 [rows, N]: row pair = w[pair] * yp of sorted row i, pair = sorted_pairs[i]; K = the intermediate size. */
+int b2q_qqq_moe_down(const int8_t* q_h, const float* s_h, const void* packed2, const float* s_channel2,
+                     const void* s_group2, const int32_t* counts, const int32_t* offsets, const int32_t* sorted_pairs,
+                     const float* pair_weights, float* ypair, int E, int rows, int active, int K, int N, int group_size,
+                     int dtype, void* stream);
+
 /* FP8 (e4m3fn, W8A16) layers on the 8-bit tiers (ABI v8).  The arithmetic of the reference's TorchFP8Linear
  * (gptqmodel/nn_modules/qlinear/fp8.py, its dequantise-then-matmul path), T = fp16 (dtype 0) or bf16 (dtype 1):
  *   W[k, n] = RN_T( float(T(w[n, k])) / float(scales[k / group_size, n]) )      (correctly rounded division)
@@ -265,6 +295,19 @@ int b2q_fp8_mm(const void* x, const void* packed, const void* scales, const void
 /* out[K, N] (T, row-major) = W of b2q_fp8_mm, exactly the operand the tensor-core tiers multiply. */
 int b2q_fp8_dequant(const void* packed, const void* scales, void* out, int K, int N, int group_size, int dtype,
                     void* stream);
+/* FP8 MoE experts (an addition to ABI v8): the grouped modes of b2q_moe_gate_up / b2q_moe_down with W = the operand of
+ * b2q_fp8_dequant.  Stacks: packed [E, b2q_packed_bytes(K, N, 8)] and scales T [E, K / group_size, N], one group_size per
+ * role.  One block is five launches with no host synchronisation: b2q_moe_align, b2q_moe_gather, b2q_fp8_moe_gate_up,
+ * b2q_fp8_moe_down, b2q_moe_combine.  The arithmetic is that of the GPTQ grouped path: g = T(x W1_e), u = T(x W3_e),
+ * h = T(T(silu(g)) * u), yp_j = T(h W2_e), y_t = T(sum_j fp32(w_j * yp_j)) (fp32 accumulation on the tensor cores).
+ * An fp16 scale table that is not finite gives zero weights, as in b2q_fp8_mm; callers refuse fp16 input for it.
+ * Envelope: that of b2q_fp8_mm, E <= 256, xs / h 16-byte aligned. */
+int b2q_fp8_moe_gate_up(const void* xs, const void* packed1, const void* scales1, const void* packed3,
+                        const void* scales3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                        int active, int K, int N, int group_size, int dtype, void* stream);
+int b2q_fp8_moe_down(const void* h, const void* packed2, const void* scales2, const int32_t* counts,
+                     const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair, int E,
+                     int rows, int active, int K, int N, int group_size, int dtype, void* stream);
 
 /* Block-FP8 (W8A8) layers of HF / DeepSeek-native checkpoints (an addition to ABI v8 that changes no earlier entry
  * point): `quant_method: fp8`, `fmt: e4m3`, `activation_scheme: dynamic`, `weight_block_size: [128, 128]` (transformers' FineGrainedFP8Config, DeepSeek-V3, the
