@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libb2q.so")
 ABI_VERSION = 8
 
 # every symbol include/b2q.h declares: (restype, argtypes)
-_vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
+_vp, _i, _sz, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_float
 SYMBOLS = {
     "b2q_version": (_i, []),
     "b2q_last_error": (ctypes.c_char_p, []),
@@ -57,6 +57,11 @@ SYMBOLS = {
     "b2q_fp8blk_quantize": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_fp8blk_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "b2q_fp8ch_workspace_bytes": (_sz, [_i, _i]),
+    "b2q_fp8ch_quantize": (_i, [_vp, _vp, _vp, _i, _i, _f, _i, _vp]),
+    "b2q_fp8ch_quantize_static": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b2q_fp8ch_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8ch_forward": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
     "b2q_fp8blk_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),

@@ -245,4 +245,22 @@ struct ET<__nv_bfloat16> {
   }
 };
 
+// ------------------------------------------------------------------------------------------------
+// e4m3 activation codes (block-FP8 and per-channel FP8 quantisers)
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// eight elements -> their eight e4m3 codes e4m3_rn_satfinite(x / s), element e in byte e
+template <typename T>
+__device__ __forceinline__ uint2 fblk_code8(const uint4& v, float s) {
+  const T* h = reinterpret_cast<const T*>(&v);
+  float q[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) q[e] = ET<T>::to_f(h[e]) / s;  // IEEE division
+  return make_uint2(e4m3x2(q[0], q[1]) | (e4m3x2(q[2], q[3]) << 16), e4m3x2(q[4], q[5]) | (e4m3x2(q[6], q[7]) << 16));
+}
+
 }  // namespace b2q

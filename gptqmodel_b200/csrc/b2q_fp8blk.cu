@@ -70,20 +70,6 @@ __device__ __forceinline__ float fblk_group_scale(const uint4& v) {
   for (int o = 8; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
   return fmaxf(a, 1e-10f) / 448.f;  // IEEE division
 }
-__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
-  uint16_t r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-// eight elements -> their eight e4m3 codes, element e in byte e
-template <typename T>
-__device__ __forceinline__ uint2 fblk_code8(const uint4& v, float s) {
-  const T* h = reinterpret_cast<const T*>(&v);
-  float q[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) q[e] = ET<T>::to_f(h[e]) / s;  // IEEE division
-  return make_uint2(e4m3x2(q[0], q[1]) | (e4m3x2(q[2], q[3]) << 16), e4m3x2(q[4], q[5]) | (e4m3x2(q[6], q[7]) << 16));
-}
 
 // one half-warp per (token m, k-block b); lane j of it owns elements 8 j .. 8 j + 7
 template <typename T>

@@ -1,0 +1,352 @@
+// b2q_fp8ch.cu — per-channel / per-tensor FP8 (W8A8) tier: e4m3 weights with one fp32 scale per output feature times
+// per-token (dynamic) or per-tensor (static) e4m3 activations on the e4m3 tensor cores (compressed-tensors FP8 /
+// FP8_DYNAMIC, fbgemm_fp8).  include/b2q.h states the arithmetic.  Kernels:
+//   * fp8ch_quant_kernel: one CTA per token row: amax over the whole row, s_x = max(min(amax, ub), 1e-10) / 448 (IEEE
+//     division), codes = e4m3_rn_satfinite(x / s_x) (fblk_code8, IEEE division), written as uint8 [M, K] and fp32 [M].
+//   * fp8ch_static_quant_kernel: elementwise codes = e4m3_rn_satfinite(x / s_in), s_x[m] = s_in.
+//   * fp8ch_gemm_kernel: the pipeline of fp8blk_gemm_kernel (b2q_fp8blk.cu) with the scales taken out of the k-loop:
+//     warp 8 loads 128 features x 128 k of the checkpoint weight [N, K] and NTOK x 128 activation codes per k-block with
+//     TMA, warpgroups 0 / 1 multiply features 0..63 / 64..127 on m64nNk32.f32.e4m3.e4m3 into a per-block fp32 P that is
+//     added to the fp32 accumulator once per k-block (acc += P).  The `ks` CTAs of a cluster split the k-blocks in
+//     contiguous runs and sum their partials over distributed shared memory in rank order; the epilogue then applies
+//     y = T(acc * (s_x[m] * s_w[n]) + bias[n]), one rounding.
+//     Static-scale decode (M <= 8, FUSED): no quantiser launch.  Warp 8 quantises each k-block it hands to the MMA warps
+//     with the layer's s_in and fblk_code8, so the codes equal fp8ch_static_quant_kernel's.  Per-token scales depend on
+//     the whole row, which a split-K rank does not read: their decode runs fp8ch_quant_kernel and the GEMM under
+//     programmatic dependent launch, which measured faster than finding the row amax inside the GEMM (DESIGN.md).
+#include <cuda.h>
+
+#include <type_traits>
+
+#include "b2q_common.cuh"
+#include "b2q_internal.h"
+#include "b2q_wgmma.cuh"
+
+namespace b2q {
+
+constexpr int C_BF = 128;                 // features per tile
+constexpr int C_BK = 128;                 // k per block (one SWIZZLE_128B row of e4m3)
+constexpr int C_MMA_THREADS = 256;        // warps 0..7: two MMA warpgroups
+constexpr int C_THREADS = C_MMA_THREADS + 32;  // + warp 8: producer
+constexpr int C_QUANT_THREADS = 256;      // quantisers
+
+template <int NTOK>
+struct FchCfg {
+  static constexpr int ST = NTOK == 128 ? 6 : 8;  // stages
+  static constexpr int W_BYTES = C_BF * C_BK;
+  static constexpr int X_BYTES = NTOK * C_BK;
+  static constexpr int STAGE_BYTES = W_BYTES + X_BYTES;
+  static constexpr int SX_BYTES = 128 * 4;  // the token scales of the CTA's rows (NTOK <= 128)
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int SMEM_BYTES = ST * STAGE_BYTES + SX_BYTES + BAR_BYTES + 1024;
+  static constexpr int ACC = NTOK / 2;
+  static_assert(STAGE_BYTES % 1024 == 0, "stages must stay 1024-byte aligned (SWIZZLE_128B atoms)");
+  static_assert(NTOK * C_BF * 4 <= ST * STAGE_BYTES, "the fp32 partial tile reuses the stages");
+  static_assert(2 * ST * 8 <= BAR_BYTES, "mbarrier area");
+  static_assert(SMEM_BYTES <= 227 * 1024, "dynamic shared memory of one CTA");
+};
+
+// ------------------------------------------------------------------------------------------------
+// quantisers
+// ------------------------------------------------------------------------------------------------
+// max |x| of eight elements
+template <typename T>
+__device__ __forceinline__ float amax8(const uint4& v) {
+  const T* h = reinterpret_cast<const T*>(&v);
+  float a = 0.f;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) a = fmaxf(a, fabsf(ET<T>::to_f(h[e])));
+  return a;
+}
+__device__ __forceinline__ float warp_max(float a) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+  return a;
+}
+
+// one CTA per token row m
+template <typename T>
+__global__ void __launch_bounds__(C_QUANT_THREADS)
+    fp8ch_quant_kernel(const T* __restrict__ x, uint8_t* __restrict__ codes, float* __restrict__ s_x, int K, float ub) {
+  __shared__ float red[C_QUANT_THREADS / 32];
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // x is the previous kernel's output
+  const size_t row = (size_t)blockIdx.x * K;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row);
+  const int n8 = K / 8;
+  float a = 0.f;
+  for (int o = threadIdx.x; o < n8; o += C_QUANT_THREADS) a = fmaxf(a, amax8<T>(xr[o]));
+  a = warp_max(a);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = a;
+  __syncthreads();
+  a = 0.f;
+#pragma unroll
+  for (int w = 0; w < C_QUANT_THREADS / 32; ++w) a = fmaxf(a, red[w]);
+  const float s = fmaxf(fminf(a, ub), 1e-10f) / 448.f;  // IEEE division; ub = +inf: no bound
+  uint2* cr = reinterpret_cast<uint2*>(codes + row);
+  for (int o = threadIdx.x; o < n8; o += C_QUANT_THREADS) cr[o] = fblk_code8<T>(xr[o], s);
+  if (threadIdx.x == 0) s_x[blockIdx.x] = s;
+}
+
+// elementwise over the M * K / 8 eight-element chunks; thread g < M also writes s_x[g] = s_in
+template <typename T>
+__global__ void __launch_bounds__(C_QUANT_THREADS)
+    fp8ch_static_quant_kernel(const T* __restrict__ x, const float* __restrict__ s_in, uint8_t* __restrict__ codes,
+                              float* __restrict__ s_x, int M, long long n8) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const long long g = (long long)blockIdx.x * C_QUANT_THREADS + threadIdx.x;
+  const float s = *s_in;
+  if (g < n8) reinterpret_cast<uint2*>(codes)[g] = fblk_code8<T>(reinterpret_cast<const uint4*>(x)[g], s);
+  if (g < M) s_x[g] = s;
+}
+
+// ------------------------------------------------------------------------------------------------
+// GEMM
+// ------------------------------------------------------------------------------------------------
+// four consecutive outputs of features nc .. nc + 3: T(acc * (sx * s_w[n]) + bias[n]), rounded once; bias [N] or nullptr
+template <typename T>
+__device__ __forceinline__ void store_scaled4(T* dst, const float* __restrict__ s_w, const T* bias, int nc, float sx,
+                                              const float (&a)[4]) {
+  using E = ET<T>;
+  const float4 sw = *reinterpret_cast<const float4*>(s_w + nc);
+  const float w4[4] = {sw.x, sw.y, sw.z, sw.w};
+  float y[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    y[i] = __fmul_rn(a[i], __fmul_rn(sx, w4[i]));  // no contraction into an fma with the bias
+    if (bias != nullptr) y[i] = __fadd_rn(y[i], E::to_f(bias[nc + i]));
+  }
+  *reinterpret_cast<uint2*>(dst) = make_uint2(E::pack2(y[0], y[1]), E::pack2(y[2], y[3]));
+}
+
+// FUSED: 0 = codes and token scales come from a quantiser kernel (TMA for the codes); 1 / 2 = M <= 8, x fp16 / bf16 is
+// quantised by the producer with the static scale s_in
+template <int NTOK, int FUSED>
+__global__ void __launch_bounds__(C_THREADS, 1)
+    fp8ch_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                      const void* __restrict__ x, const float* __restrict__ s_x, const float* __restrict__ s_in,
+                      const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M, int K,
+                      int N, int kpc, int out_bf16) {
+  using C = FchCfg<NTOK>;
+  constexpr int ST = C::ST;
+  static_assert(!FUSED || NTOK == 8, "the fused quantiser serves 8-token tiles");
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  // stage s: [W 128 x 128][X NTOK x 128]; then the token scales and the barriers
+  float* sxr = reinterpret_cast<float*>(smem + ST * C::STAGE_BYTES);
+  const uint32_t bar_full = smem_base + ST * C::STAGE_BYTES + C::SX_BYTES, bar_empty = bar_full + 8 * ST;
+  auto sW = [&](int s) { return smem_base + (uint32_t)(s * C::STAGE_BYTES); };
+  auto sX = [&](int s) { return sW(s) + C::W_BYTES; };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n0 = blockIdx.x * C_BF;
+  const int row0 = blockIdx.z * NTOK, rows = min(NTOK, M - row0);
+  const int KB = K / C_BK;
+  const uint32_t nrank = cluster_nctarank(), crank = cluster_ctarank();
+  const int kb0 = min(KB, (int)crank * kpc), kb1 = min(KB, kb0 + kpc);
+  const int nkb = kb1 - kb0;
+
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_w);
+    if (!FUSED) prefetch_tmap(&tmap_q);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(bar_full + 8 * s, FUSED ? 32 : 1);
+      mbar_init(bar_empty + 8 * s, C_MMA_THREADS / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  auto load_weights = [&](int i, int s) {
+    mbar_expect_tx_only(bar_full + 8 * s, C::W_BYTES);
+    tma_load_2d(sW(s), &tmap_w, bar_full + 8 * s, (kb0 + i) * C_BK, n0);
+  };
+  // the weight stream of the first ST blocks starts at once (under programmatic dependent launch: while the previous
+  // kernel still runs)
+  if (warp == 8 && lane == 0)
+    for (int i = 0; i < nkb && i < ST; ++i) load_weights(i, i);
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // x / codes / s_x are the previous kernels' output
+
+  // the scales of the CTA's token rows -> sxr (rows past M: 0)
+  if (!FUSED) {
+    for (int t = threadIdx.x; t < NTOK; t += C_THREADS) sxr[t] = t < rows ? s_x[row0 + t] : 0.f;
+  } else if (threadIdx.x < NTOK) {
+    sxr[threadIdx.x] = (int)threadIdx.x < M ? *s_in : 0.f;
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    // ================================ producer ================================
+    if (FUSED) {
+      using T = typename std::conditional<FUSED == 1, __half, __nv_bfloat16>::type;
+      // half-warp h of pass p holds token t = 2 p + h, lane j = lane & 15 its elements 8 j .. 8 j + 7 of the k-block;
+      // rows t >= M keep the zero codes written here once
+      constexpr int PD = 4;  // k-blocks of activations in flight ahead of the one being quantised
+      const int h = lane >> 4, j = lane & 15;
+      for (int s = 0; s < ST; ++s)
+        for (int o = lane; o < C::X_BYTES / 16; o += 32)
+          asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(sX(s) + 16u * o), "r"(0u) : "memory");
+      float sc[4];
+#pragma unroll
+      for (int p = 0; p < 4; ++p) sc[p] = sxr[2 * p + h];
+      const T* xr = reinterpret_cast<const T*>(x) + (size_t)kb0 * C_BK + 8 * j;
+      uint4 buf[PD][4];  // [in-flight k-block][pass]
+      auto fetch = [&](int i, uint4(&dst)[4]) {
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const int t = 2 * p + h;
+          dst[p] = (t < M && i < nkb) ? *reinterpret_cast<const uint4*>(xr + (size_t)t * K + (size_t)i * C_BK)
+                                      : make_uint4(0u, 0u, 0u, 0u);
+        }
+      };
+#pragma unroll
+      for (int u = 0; u < PD; ++u) fetch(u, buf[u]);
+      for (int i0 = 0; i0 < nkb; i0 += PD) {
+#pragma unroll
+        for (int u = 0; u < PD; ++u) {
+          const int i = i0 + u;
+          if (i >= nkb) break;
+          const int s = i % ST;
+          uint4 cur[4];
+#pragma unroll
+          for (int p = 0; p < 4; ++p) cur[p] = buf[u][p];
+          fetch(i + PD, buf[u]);
+          if (i >= ST) {
+            mbar_wait(bar_empty + 8 * s, ((i / ST) & 1) ^ 1);
+            if (lane == 0) load_weights(i, s);
+          }
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            const int t = 2 * p + h;
+            if (t < M) {
+              const uint2 q = fblk_code8<T>(cur[p], sc[p]);
+              const uint32_t addr = sX(s) + (uint32_t)t * 128 + ((((uint32_t)(j >> 1)) ^ (uint32_t)t) << 4) + 8u * (j & 1);
+              asm volatile("st.shared.v2.u32 [%0], {%1,%2};" ::"r"(addr), "r"(q.x), "r"(q.y) : "memory");
+            }
+          }
+          fence_proxy_async_smem();
+          mbar_arrive(bar_full + 8 * s);
+        }
+      }
+    } else if (lane == 0) {
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % ST;
+        if (i >= ST) {
+          mbar_wait(bar_empty + 8 * s, ((i / ST) & 1) ^ 1);
+          load_weights(i, s);
+        }
+        mbar_expect_tx(bar_full + 8 * s, C::X_BYTES);
+        tma_load_2d(sX(s), &tmap_q, bar_full + 8 * s, (kb0 + i) * C_BK, row0);
+      }
+    }
+  } else {
+    // ================================ MMA warpgroups ================================
+    const int wg = warp >> 2;  // features 64 wg .. 64 wg + 63 of the tile
+    float acc[C::ACC], p[C::ACC];
+#pragma unroll
+    for (int v = 0; v < C::ACC; ++v) acc[v] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % ST;
+      mbar_wait(bar_full + 8 * s, (i / ST) & 1);
+      const uint64_t wdesc = wgmma_desc_k_sw128(sW(s)) + 512 * wg;
+      const uint64_t xdesc = wgmma_desc_k_sw128(sX(s));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < C_BK / 32; ++k) Wgmma8F<NTOK>::mma(p, wdesc + 2 * k, xdesc + 2 * k, k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(p);
+      // promotion: the block's product joins the fp32 accumulator (no per-block scale)
+#pragma unroll
+      for (int v = 0; v < C::ACC; ++v) acc[v] += p[v];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+    }
+    // both warpgroups are done with the stages before either overwrites them with its partial tile
+    asm volatile("bar.sync 1, %0;" ::"r"(C_MMA_THREADS) : "memory");
+    park_partial(smem_base, wg, warp & 3, acc);
+  }
+  __syncwarp();
+  cluster_sync_all();
+  if (warp < C_MMA_THREADS / 32) {
+    // rank z reduces token rows z, z + nrank, ... , a warp per row
+    const int nc = n0 + lane * 4;
+    if (nc < N) {
+      for (int tok = (int)crank + (int)nrank * warp; tok < rows; tok += (int)nrank * (C_MMA_THREADS / 32)) {
+        float a[1][4];
+        dsmem_sum4<1, false>(smem_base + (uint32_t)tok * (C_BF * 4) + (uint32_t)lane * 16, 0, nrank, a);
+        const size_t o = (size_t)(row0 + tok) * N + nc;
+        if (out_bf16)
+          store_scaled4(reinterpret_cast<__nv_bfloat16*>(out) + o, s_w, reinterpret_cast<const __nv_bfloat16*>(bias),
+                        nc, sxr[tok], a[0]);
+        else
+          store_scaled4(reinterpret_cast<__half*>(out) + o, s_w, reinterpret_cast<const __half*>(bias), nc, sxr[tok],
+                        a[0]);
+      }
+    }
+  }
+  __syncwarp();
+  cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
+}
+
+// ------------------------------------------------------------------------------------------------
+// host side
+// ------------------------------------------------------------------------------------------------
+int launch_fp8ch_quant(const void* x, void* codes, float* s_x, int M, int K, float ub, int dtype, cudaStream_t stream) {
+  const dim3 grid((unsigned)M, 1, 1), block(C_QUANT_THREADS, 1, 1);
+  if (dtype == 0)
+    return launch_kernel(fp8ch_quant_kernel<__half>, grid, block, 0, stream, 0, true, (const __half*)x, (uint8_t*)codes,
+                         s_x, K, ub);
+  return launch_kernel(fp8ch_quant_kernel<__nv_bfloat16>, grid, block, 0, stream, 0, true, (const __nv_bfloat16*)x,
+                       (uint8_t*)codes, s_x, K, ub);
+}
+
+int launch_fp8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                              cudaStream_t stream) {
+  const long long n8 = (long long)M * (K / 8), threads = n8 > M ? n8 : M;
+  const dim3 grid((unsigned)((threads + C_QUANT_THREADS - 1) / C_QUANT_THREADS), 1, 1), block(C_QUANT_THREADS, 1, 1);
+  if (dtype == 0)
+    return launch_kernel(fp8ch_static_quant_kernel<__half>, grid, block, 0, stream, 0, true, (const __half*)x, s_in,
+                         (uint8_t*)codes, s_x, M, n8);
+  return launch_kernel(fp8ch_static_quant_kernel<__nv_bfloat16>, grid, block, 0, stream, 0, true,
+                       (const __nv_bfloat16*)x, s_in, (uint8_t*)codes, s_x, M, n8);
+}
+
+template <int NTOK, int FUSED>
+static int launch_fp8ch_gemm_t(const Fp8ChArgs& a, const SwapPlan& p) {
+  using C = FchCfg<NTOK>;
+  CUtensorMap tw, tq;
+  if (make_tmap_2d(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, a.N, (size_t)a.K, C_BK, C_BF,
+                   CU_TENSOR_MAP_SWIZZLE_128B) != 0)
+    return -1;
+  if (FUSED) {
+    tq = tw;  // unused
+  } else if (make_tmap_2d(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, C_BK, NTOK,
+                          CU_TENSOR_MAP_SWIZZLE_128B) != 0) {
+    return -1;
+  }
+  auto kern = fp8ch_gemm_kernel<NTOK, FUSED>;
+  static int smem_opted[32] = {};
+  if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8ch")) return e;
+  return launch_kernel(kern, dim3((a.N + C_BF - 1) / C_BF, p.ks, p.tblocks), dim3(C_THREADS, 1, 1), C::SMEM_BYTES,
+                       a.stream, p.ks, true, tw, tq, a.x, a.s_x, a.s_in, a.s_w, a.bias, a.out, a.M, a.K, a.N, p.kpc,
+                       a.dtype);
+}
+
+// the launch plan of the block-FP8 GEMM (same tiles, token blocks and split-K ranks)
+int launch_fp8ch_gemm(const Fp8ChArgs& a) {
+  const SwapPlan p = fp8blk_plan(0, a.M, a.K, a.N, 1, a.ks);
+  if (a.x != nullptr) return a.dtype == 0 ? launch_fp8ch_gemm_t<8, 1>(a, p) : launch_fp8ch_gemm_t<8, 2>(a, p);
+  switch (p.ntok) {
+    case 8: return launch_fp8ch_gemm_t<8, 0>(a, p);
+    case 16: return launch_fp8ch_gemm_t<16, 0>(a, p);
+    case 32: return launch_fp8ch_gemm_t<32, 0>(a, p);
+    case 64: return launch_fp8ch_gemm_t<64, 0>(a, p);
+    default: return launch_fp8ch_gemm_t<128, 0>(a, p);
+  }
+}
+
+}  // namespace b2q

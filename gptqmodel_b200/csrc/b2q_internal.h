@@ -111,6 +111,23 @@ struct Fp8BlkMoe {
 int launch_fp8blk_moe(int mode, const Fp8BlkArgs& a, const Fp8BlkMoe& g);
 int launch_fp8blk_moe_gather(const void* x, const int32_t* sorted_pairs, void* codes, float* s_x, int rows, int top_k,
                              int K, int dtype, cudaStream_t stream);
+// per-channel / per-tensor FP8 (W8A8) tier (b2q_fp8ch.cu)
+struct Fp8ChArgs {
+  const void* x;          // fused decode (M <= 8): the activations [M, K]; else nullptr
+  const void* codes;      // e4m3 codes [M, K] (x == nullptr)
+  const float* s_x;       // token scales [M] (x == nullptr)
+  const float* s_in;      // fused decode: the static input scale [1]
+  const void* weight;     // e4m3 [N, K], the checkpoint tensor
+  const float* s_w;       // [N]
+  const void* bias;       // [N] in the output dtype, or nullptr
+  void* out;              // [M, N]
+  int M, K, N, dtype, ks;  // ks <= 0: heuristic
+  cudaStream_t stream;
+};
+int launch_fp8ch_quant(const void* x, void* codes, float* s_x, int M, int K, float ub, int dtype, cudaStream_t stream);
+int launch_fp8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                              cudaStream_t stream);
+int launch_fp8ch_gemm(const Fp8ChArgs& a);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

@@ -314,6 +314,176 @@ def load_block_fp8_linears(path: str, device="cuda", dtype: Optional[torch.dtype
     return mods
 
 
+@dataclass
+class Fp8W8A8Spec:
+    """A per-channel / per-tensor FP8 (W8A8) config: compressed-tensors `float-quantized` or transformers' fbgemm_fp8.
+    kv_cache_scheme is the checkpoint's KV-cache quantisation, returned untouched: the attention that would apply it is
+    the caller's, not this package's."""
+    method: str                       # "compressed-tensors" | "fbgemm_fp8"
+    weight_strategy: str = "channel"  # "channel" | "tensor"
+    activation: str = "dynamic"       # "dynamic" (per token) | "static" (per tensor, input_scale)
+    ub: Optional[float] = None        # fbgemm_fp8: activation_scale_ub
+    ignore: tuple = ()                # compressed-tensors: names / "re:" patterns; fbgemm_fp8: name fragments
+    kv_cache_scheme: Optional[dict] = None
+
+    def ignores(self, name: str) -> bool:
+        if self.method == "fbgemm_fp8":  # transformers' modules_to_not_convert: a fragment of the module's name
+            return any(k in name for k in self.ignore)
+        return any(re.match(k[3:], name) if k.startswith("re:") else k == name for k in self.ignore)
+
+
+def _ct_args(where: str, a, kinds) -> tuple:
+    """(strategy, dynamic) of one compressed-tensors QuantizationArgs dict that this package serves."""
+    if not isinstance(a, dict):
+        raise ValueError(f"compressed-tensors: `{where}` must be a dict, got {a!r}")
+    nb, typ, sym, strat, dyn = (a.get(k) for k in ("num_bits", "type", "symmetric", "strategy", "dynamic"))
+    if not isinstance(nb, int) or isinstance(nb, bool) or nb <= 0:
+        raise ValueError(f"compressed-tensors: `{where}.num_bits` must be a positive integer, got {nb!r}")
+    if typ not in ("int", "float") or not isinstance(sym, bool) or not isinstance(strat, str):
+        raise ValueError(f"compressed-tensors: `{where}` needs type int | float, a boolean `symmetric` and a `strategy`")
+    if not (isinstance(dyn, bool) or dyn == "local"):
+        raise ValueError(f"compressed-tensors: `{where}.dynamic` must be a boolean, got {dyn!r}")
+    if typ != "float" or nb != 8:
+        raise NotImplementedError(f"compressed-tensors: {where} of {nb}-bit {typ} are not served (8-bit float only)")
+    if not sym:
+        raise NotImplementedError(f"compressed-tensors: asymmetric {where} are not served")
+    if strat not in ("tensor", "channel", "group", "block", "token", "tensor_group", "attn_head"):
+        raise ValueError(f"compressed-tensors: unknown `{where}.strategy` `{strat}`")
+    if (strat, dyn) not in kinds:
+        raise NotImplementedError(f"compressed-tensors: {where} with strategy `{strat}`, dynamic={dyn} are not served "
+                                  f"(served: {', '.join(f'{s} / dynamic={d}' for s, d in kinds)})")
+    return strat, dyn
+
+
+def parse_fp8_w8a8_config(raw: dict) -> Fp8W8A8Spec:
+    """Per-channel / per-tensor FP8 (W8A8) configs:
+      * `quant_method: compressed-tensors`, `format: float-quantized`; every config group targets ["Linear"] with weights
+        {num_bits: 8, type: float, symmetric: true, dynamic: false, strategy: channel | tensor} and input activations
+        {num_bits: 8, type: float, symmetric: true} either {strategy: token, dynamic: true} or {strategy: tensor,
+        dynamic: false}, the same in every group.  `ignore` holds module names and `re:` patterns;
+      * `quant_method: fbgemm_fp8` with `activation_scale_ub` (default 1200.0) and `modules_to_not_convert`.
+    NotImplementedError for what the kernels do not serve (group / block strategies, int types, asymmetric or dynamic
+    weights, mixed groups, other targets or formats), ValueError for malformed entries."""
+    if not isinstance(raw, dict):
+        raise ValueError(f"FP8 W8A8: the quantisation config must be a dict, got {type(raw).__name__}")
+    method = raw.get("quant_method")
+    if method == "fbgemm_fp8":
+        ub = raw.get("activation_scale_ub", 1200.0)
+        if isinstance(ub, bool) or not isinstance(ub, (int, float)) or not (0.0 < float(ub) < float("inf")):
+            raise ValueError(f"fbgemm_fp8: `activation_scale_ub` must be a positive number, got {ub!r}")
+        skip = raw.get("modules_to_not_convert") or []
+        if not (isinstance(skip, (list, tuple)) and all(isinstance(s, str) for s in skip)):
+            raise ValueError(f"fbgemm_fp8: `modules_to_not_convert` must be a list of names, got {skip!r}")
+        return Fp8W8A8Spec("fbgemm_fp8", "channel", "dynamic", float(ub), tuple(skip))
+    if method != "compressed-tensors":
+        raise NotImplementedError(f"FP8 W8A8: quant_method `{method}` is not compressed-tensors or fbgemm_fp8")
+    fmt = raw.get("format")
+    if fmt != "float-quantized":
+        raise NotImplementedError(f"compressed-tensors: format `{fmt}` is not served (float-quantized only)")
+    groups = raw.get("config_groups")
+    if not isinstance(groups, dict) or not groups:
+        raise ValueError("compressed-tensors: `config_groups` must be a non-empty dict")
+    kinds = set()
+    for gname, g in groups.items():
+        if not isinstance(g, dict):
+            raise ValueError(f"compressed-tensors: config group `{gname}` must be a dict")
+        targets = g.get("targets")
+        if not (isinstance(targets, list) and all(isinstance(t, str) for t in targets)):
+            raise ValueError(f"compressed-tensors: `{gname}.targets` must be a list of names")
+        if targets != ["Linear"]:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` targets {targets} (only [\"Linear\"] is served)")
+        if g.get("format") not in (None, "float-quantized"):
+            raise NotImplementedError(f"compressed-tensors: `{gname}` has format `{g.get('format')}`")
+        if g.get("output_activations") is not None:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` quantises output activations")
+        if g.get("weights") is None or g.get("input_activations") is None:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` is not W8A8 (weights and input activations)")
+        ws, _ = _ct_args(f"{gname}.weights", g["weights"], {("channel", False), ("tensor", False)})
+        _, dyn = _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True), ("tensor", False)})
+        kinds.add((ws, "dynamic" if dyn else "static"))
+    if len(kinds) != 1:
+        raise NotImplementedError(f"compressed-tensors: mixed config groups {sorted(kinds)} are not served")
+    ignore = raw.get("ignore") or []
+    if not (isinstance(ignore, (list, tuple)) and all(isinstance(s, str) for s in ignore)):
+        raise ValueError(f"compressed-tensors: `ignore` must be a list of names, got {ignore!r}")
+    for k in ignore:
+        if k.startswith("re:"):
+            try:
+                re.compile(k[3:])
+            except re.error as e:
+                raise ValueError(f"compressed-tensors: bad `ignore` pattern `{k}`: {e}") from None
+    kv = raw.get("kv_cache_scheme")
+    if kv is not None and not isinstance(kv, dict):
+        raise ValueError(f"compressed-tensors: `kv_cache_scheme` must be a dict, got {kv!r}")
+    (ws, act), = kinds
+    return Fp8W8A8Spec("compressed-tensors", ws, act, None, tuple(ignore), kv)
+
+
+@torch.no_grad()
+def load_fp8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype] = None,
+                          only: Optional[Iterable[str]] = None,
+                          post_init: Optional[bool] = None) -> Dict[str, nn.Module]:
+    """Load every FP8 W8A8 linear of a compressed-tensors FP8 / FP8_DYNAMIC or fbgemm_fp8 checkpoint into
+    B200ChannelFp8Linear modules.
+
+    Modules are the `<prefix>.weight` + `<prefix>.weight_scale` pairs that the config does not ignore; the rest (an
+    unquantised lm_head, norms, embeddings) stay dense and are not returned.  A static layer must carry its
+    `input_scale` and a dynamic one must not (NotImplementedError); shapes are checked (ValueError).
+    only      : optional iterable of module prefixes to load (default: all found)
+    post_init : default True on CUDA devices, False on CPU (tensors only; host tests)
+    """
+    from safetensors import safe_open
+
+    from .fp8_channel import B200ChannelFp8Linear
+
+    spec = parse_fp8_w8a8_config(_read_raw_config(path))
+    wmap = _weight_map(path)
+    if only is not None:
+        prefixes = list(only)
+    else:
+        sfx = ".weight_scale"
+        prefixes = sorted(n[: -len(sfx)] for n in wmap if n.endswith(sfx) and n[: -len(sfx)] + ".weight" in wmap)
+        prefixes = [p for p in prefixes if not spec.ignores(p)]
+    dev = torch.device(device)
+    do_post = (dev.type == "cuda") if post_init is None else post_init
+    handles: Dict[str, object] = {}
+
+    def tensor(name):
+        fn = wmap.get(name)
+        if fn is None:
+            return None
+        if fn not in handles:
+            handles[fn] = safe_open(fn, framework="pt").__enter__()
+        return handles[fn].get_tensor(name)
+
+    mods: Dict[str, nn.Module] = {}
+    try:
+        for prefix in prefixes:
+            t = {s: tensor(f"{prefix}.{s}") for s in ("weight", "weight_scale", "input_scale", "bias")}
+            if t["weight"] is None or t["weight_scale"] is None:
+                raise KeyError(f"{prefix}: checkpoint misses weight / weight_scale")
+            if t["weight"].dtype != torch.float8_e4m3fn:
+                raise NotImplementedError(f"{prefix}: weight dtype {t['weight'].dtype} is not served "
+                                          "(float8_e4m3fn only)")
+            if spec.activation == "static" and t["input_scale"] is None:
+                raise NotImplementedError(f"{prefix}: static activations need `input_scale`, the checkpoint has none")
+            if spec.activation == "dynamic" and t["input_scale"] is not None:
+                raise NotImplementedError(f"{prefix}: `input_scale` on a layer with dynamic activations")
+            ws = t["weight_scale"]
+            if spec.weight_strategy == "tensor" and ws.numel() != 1:
+                raise ValueError(f"{prefix}: per-tensor weight_scale has shape {tuple(ws.shape)}")
+            mods[prefix] = B200ChannelFp8Linear.from_checkpoint_tensors(
+                t["weight"], ws, input_scale=t["input_scale"], bias=t["bias"], activation=spec.activation,
+                ub=spec.ub, device=dev, dtype=dtype, post_init=do_post, name=prefix)
+    finally:
+        for h in handles.values():
+            close = getattr(h, "__exit__", None)
+            if close is not None:
+                close(None, None, None)
+        handles.clear()
+    return mods
+
+
 def _weight_map(path: str) -> Dict[str, str]:
     """tensor name -> safetensors file (single file or sharded with model.safetensors.index.json)."""
     idx = os.path.join(path, "model.safetensors.index.json")

@@ -340,6 +340,45 @@ int b2q_fp8blk_mm(const void* codes, const float* s_x, const void* weight, const
 int b2q_fp8blk_forward(const void* x, const void* weight, const float* s_w, const void* bias, void* out, int M, int K,
                        int N, int dtype, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Per-channel FP8 (W8A8) layers (an addition to ABI v8 that changes no earlier entry point): compressed-tensors
+ * `float-quantized` FP8_DYNAMIC (channel weights, dynamic per-token activations) and FP8 (tensor weights, a static
+ * per-tensor input_scale), and transformers' fbgemm_fp8 (channel weights, per-token activations with amax bounded by
+ * activation_scale_ub).  Weights e4m3 w [N, K] (the checkpoint tensor, unchanged), s_w fp32 [N], one scale per output
+ * feature that MULTIPLIES the weights (a per-tensor scale is broadcast to [N] by the caller).  T = fp16 (dtype 0) or bf16
+ * (dtype 1), KB = K / 128.  For every token row m:
+ *   dynamic: s_x[m] = fmaxf(fminf(max_k |x[m,k]|, ub), 1e-10f) / 448.f     (ub = +inf: no bound; IEEE fp32 division)
+ *   static:  s_x[m] = s_in                                                   (the layer's input_scale)
+ *   q[m,k]   = e4m3_rn_satfinite(float(x[m,k]) / s_x[m])                    (IEEE fp32 division)
+ *   P_b[m,n] = sum_{k in b} q[m,k] * w[n,k]                                 (e4m3 wgmma, fp32 accumulation)
+ *   acc[m,n] = acc[m,n] + P_b[m,n]                                           for b in increasing order, from 0
+ *   y        = T((acc * (s_x[m] * s_w[n])) + bias[n])                       (fp32 products and sum, NOT fused; one
+ *                                                                             rounding to T; bias optional, T [N])
+ * The bias is added before the one rounding (fbgemm rounds the product first and adds the bias in T).  The fp8
+ * tensor-core accumulator is not an exact fp32 sum, so P_b is not exact in general; it joins the fp32 accumulator once
+ * per 128-k block.  Split-K: each of the `ks` ranks of a tile sums its own contiguous run of k-blocks in order from 0,
+ * and the ranks' fp32 partials are added in rank order before the epilogue.  Deterministic for a launch plan.
+ * Envelope: that of block-FP8 (K % 128 == 0, K <= 65536, N % 64 == 0); x, codes, weight, s_w, out, workspace and the
+ * quantisers' s_x 16-byte aligned.  Bad arguments return -2 before any CUDA work. */
+/* Workspace of b2q_fp8ch_forward for M rows: the codes and token scales (unused by a static-scale layer at M <= 8). */
+size_t b2q_fp8ch_workspace_bytes(int M, int K);
+/* Dynamic per-token quantiser: x T [M, K] -> codes e4m3 [M, K], s_x fp32 [M]; ub > 0 (+inf: no bound).  Launched with
+ * programmatic dependent launch, like b2q_fp8blk_quantize. */
+int b2q_fp8ch_quantize(const void* x, void* codes, float* s_x, int M, int K, float ub, int dtype, void* stream);
+/* Static quantiser: codes = e4m3_rn_satfinite(x / s_in) with s_in a device fp32 [1]; s_x[m] = s_in for every row. */
+int b2q_fp8ch_quantize_static(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                              void* stream);
+/* out T [M, N] from either quantiser's codes and scales; ks = split-K ranks (1..8), <= 0: the heuristic (the plan of
+ * b2q_fp8blk_mm). */
+int b2q_fp8ch_mm(const void* codes, const float* s_x, const void* weight, const float* s_w, const void* bias, void* out,
+                 int M, int K, int N, int dtype, int ks, void* stream);
+/* The layer: s_in != NULL selects static scales, else dynamic per-token scales bounded by ub.  Static scales at M <= 8
+ * run in ONE launch that quantises the activation blocks it consumes (the codes of b2q_fp8ch_quantize_static, the plan
+ * of b2q_fp8ch_mm with ks <= 0, so the output is identical to theirs); otherwise a quantiser + b2q_fp8ch_mm through the
+ * workspace under programmatic dependent launch.  Dispatches on M inside the library, so a CUDA graph sees the true M. */
+int b2q_fp8ch_forward(const void* x, const void* weight, const float* s_w, const float* s_in, float ub,
+                      const void* bias, void* out, int M, int K, int N, int dtype, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* Block-FP8 MoE experts (an addition to ABI v8): the experts' w1 / w3 [E*I, K], w2 [E*H, I] e4m3 stacks and their scale
  * stacks [E, ceil(N/128), K/128] (each expert's checkpoint tensors, back to back), the routing tables of b2q_moe_align.
  * One block is six launches with no host synchronisation: b2q_moe_align, b2q_fp8blk_moe_gather, b2q_fp8blk_moe_gate_up,
