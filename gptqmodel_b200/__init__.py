@@ -7,6 +7,7 @@ Public API:
     B200Fp8QuantLinear  FP8 (e4m3fn, W8A16) checkpoints on the 8-bit tiers
     B200BlockFp8Linear  HF / DeepSeek-native block-FP8 (W8A8) checkpoints on the e4m3 tensor cores
     B200ChannelFp8Linear  per-channel / per-tensor FP8 (W8A8: compressed-tensors FP8 / FP8_DYNAMIC, fbgemm_fp8)
+    B200ChannelInt8Linear per-channel / per-tensor INT8 (W8A8: compressed-tensors int-quantized) on the s8 tensor cores
     lib / check       the raw C-ABI (include/b2q.h) through ctypes
 """
 from ._lib import ABI_VERSION, B2QError, LIB_PATH, SYMBOLS, check, lib  # noqa: F401
@@ -17,5 +18,6 @@ from .qqq import B200QqqQuantLinear  # noqa: F401
 from .fp8 import B200Fp8QuantLinear  # noqa: F401
 from .fp8_block import B200BlockFp8Linear  # noqa: F401
 from .fp8_channel import B200ChannelFp8Linear  # noqa: F401
+from .int8_channel import B200ChannelInt8Linear  # noqa: F401
 
-__all__ = ["B200QuantLinear", "B200AwqQuantLinear", "B200QqqQuantLinear", "B200Fp8QuantLinear", "B200BlockFp8Linear", "B200ChannelFp8Linear", "awq_gemm_to_gptq", "Lora", "fuse_siblings", "SiblingGroup", "lib", "check", "B2QError", "LIB_PATH", "SYMBOLS", "ABI_VERSION"]
+__all__ = ["B200QuantLinear", "B200AwqQuantLinear", "B200QqqQuantLinear", "B200Fp8QuantLinear", "B200BlockFp8Linear", "B200ChannelFp8Linear", "B200ChannelInt8Linear", "awq_gemm_to_gptq", "Lora", "fuse_siblings", "SiblingGroup", "lib", "check", "B2QError", "LIB_PATH", "SYMBOLS", "ABI_VERSION"]

@@ -864,6 +864,75 @@ int b2q_fp8ch_forward(const void* x, const void* weight, const float* s_w, const
   return check_cuda(launch_fp8ch_gemm(a), "b2q_fp8ch_forward");
 }
 
+// ---- per-channel / per-tensor INT8 (compressed-tensors int-quantized W8A8) tier: the GEMM of b2q_fp8ch on s8 ----
+size_t b2q_int8ch_workspace_bytes(int M, int K) { return b2q_fp8ch_workspace_bytes(M, K); }
+
+int b2q_int8ch_quantize(const void* x, void* codes, float* s_x, int M, int K, int dtype, void* stream) {
+  if (int e = fp8blk_check_shape("b2q_int8ch_quantize", M, K, 64, dtype)) return e;
+  if (M == 0) return 0;
+  if (x == nullptr || codes == nullptr || s_x == nullptr || !aligned16(x) || !aligned16(codes) || !aligned16(s_x)) {
+    set_error("b2q_int8ch_quantize: x, codes and s_x must be 16-byte aligned device pointers");
+    return -2;
+  }
+  DeviceGuard dg(codes);
+  return check_cuda(launch_int8ch_quant(x, codes, s_x, M, K, dtype, (cudaStream_t)stream), "b2q_int8ch_quantize");
+}
+
+int b2q_int8ch_quantize_static(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                               void* stream) {
+  if (int e = fp8blk_check_shape("b2q_int8ch_quantize_static", M, K, 64, dtype)) return e;
+  if (M == 0) return 0;
+  if (x == nullptr || s_in == nullptr || codes == nullptr || s_x == nullptr || !aligned16(x) || !aligned16(codes) ||
+      !aligned16(s_x)) {
+    set_error("b2q_int8ch_quantize_static: x, s_in, codes and s_x must be device pointers, x, codes and s_x 16-byte "
+              "aligned");
+    return -2;
+  }
+  DeviceGuard dg(codes);
+  return check_cuda(launch_int8ch_static_quant(x, s_in, codes, s_x, M, K, dtype, (cudaStream_t)stream),
+                    "b2q_int8ch_quantize_static");
+}
+
+int b2q_int8ch_mm(const void* codes, const float* s_x, const void* weight, const float* s_w, const void* bias, void* out,
+                  int M, int K, int N, int dtype, int ks, void* stream) {
+  if (int e = fp8blk_check_shape("b2q_int8ch_mm", M, K, N, dtype)) return e;
+  if (int e = fp8blk_check_layer("b2q_int8ch_mm", weight, s_w, out)) return e;
+  if (ks > 8) {
+    set_error("b2q_int8ch_mm: ks=%d exceeds the cluster limit 8", ks);
+    return -2;
+  }
+  if (M == 0) return 0;
+  if (codes == nullptr || s_x == nullptr || !aligned16(codes)) {
+    set_error("b2q_int8ch_mm: codes (16-byte aligned) and s_x must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(weight);
+  Fp8ChArgs a = {nullptr, codes, s_x, nullptr, weight, s_w, bias, out, M, K, N, dtype, ks, (cudaStream_t)stream};
+  return check_cuda(launch_int8ch_gemm(a), "b2q_int8ch_mm");
+}
+
+int b2q_int8ch_forward(const void* x, const void* weight, const float* s_w, const float* s_in, const void* bias,
+                       void* out, int M, int K, int N, int dtype, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+  if (int e = fp8blk_check_shape("b2q_int8ch_forward", M, K, N, dtype)) return e;
+  if (int e = fp8blk_check_layer("b2q_int8ch_forward", weight, s_w, out)) return e;
+  if (M == 0) return 0;
+  const size_t need = b2q_int8ch_workspace_bytes(M, K);
+  if (x == nullptr || !aligned16(x) || workspace == nullptr || !aligned16(workspace) || workspace_bytes < need) {
+    set_error("b2q_int8ch_forward: x and a workspace of b2q_int8ch_workspace_bytes(M, K) = %zu bytes (16-byte "
+              "aligned) must be given, got %zu", need, workspace_bytes);
+    return -2;
+  }
+  DeviceGuard dg(weight);
+  int8_t* codes = reinterpret_cast<int8_t*>(workspace);
+  float* s_x = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + fp8blk_codes_bytes(M, K));
+  int e = s_in != nullptr ? launch_int8ch_static_quant(x, s_in, codes, s_x, M, K, dtype, (cudaStream_t)stream)
+                          : launch_int8ch_quant(x, codes, s_x, M, K, dtype, (cudaStream_t)stream);
+  if ((e = check_cuda(e, "b2q_int8ch_forward")) != 0) return e;
+  Fp8ChArgs a = {nullptr, codes, s_x, nullptr, weight, s_w, bias, out, M, K, N, dtype, 0, (cudaStream_t)stream};
+  return check_cuda(launch_int8ch_gemm(a), "b2q_int8ch_forward");
+}
+
 // ---- block-FP8 MoE experts: the grouped modes of fp8blk_gemm_kernel over the routing tables of b2q_moe_align ----
 static int fp8blk_moe_check(const char* fn, const void* codes, const float* s_x, const void* w, const float* s_w,
                             const void* out, const int32_t* counts, const int32_t* offsets, int E, int rows, int K, int N,

@@ -1,19 +1,26 @@
-// b2q_fp8ch.cu — per-channel / per-tensor FP8 (W8A8) tier: e4m3 weights with one fp32 scale per output feature times
-// per-token (dynamic) or per-tensor (static) e4m3 activations on the e4m3 tensor cores (compressed-tensors FP8 /
-// FP8_DYNAMIC, fbgemm_fp8).  include/b2q.h states the arithmetic.  Kernels:
+// b2q_fp8ch.cu — per-channel / per-tensor 8-bit W8A8 tier: 8-bit weights with one fp32 scale per output feature times
+// per-token (dynamic) or per-tensor (static) 8-bit activations on the 8-bit tensor cores.  Two formats share the GEMM:
+// e4m3 (compressed-tensors FP8 / FP8_DYNAMIC, fbgemm_fp8) and int8 (compressed-tensors int-quantized W8A8).
+// include/b2q.h states the arithmetic of both.  Kernels:
 //   * fp8ch_quant_kernel: one CTA per token row: amax over the whole row, s_x = max(min(amax, ub), 1e-10) / 448 (IEEE
 //     division), codes = e4m3_rn_satfinite(x / s_x) (fblk_code8, IEEE division), written as uint8 [M, K] and fp32 [M].
 //   * fp8ch_static_quant_kernel: elementwise codes = e4m3_rn_satfinite(x / s_in), s_x[m] = s_in.
+//   * int8ch_quant_kernel / int8ch_static_quant_kernel: the same two with s_x = max(amax, 1e-10) / 127 and int8 codes
+//     clamp(rint(x / s_x), -128, 127) (int8_code8).
 //   * fp8ch_gemm_kernel: the pipeline of fp8blk_gemm_kernel (b2q_fp8blk.cu) with the scales taken out of the k-loop:
 //     warp 8 loads 128 features x 128 k of the checkpoint weight [N, K] and NTOK x 128 activation codes per k-block with
 //     TMA, warpgroups 0 / 1 multiply features 0..63 / 64..127 on m64nNk32.f32.e4m3.e4m3 into a per-block fp32 P that is
 //     added to the fp32 accumulator once per k-block (acc += P).  The `ks` CTAs of a cluster split the k-blocks in
 //     contiguous runs and sum their partials over distributed shared memory in rank order; the epilogue then applies
 //     y = T(acc * (s_x[m] * s_w[n]) + bias[n]), one rounding.
-//     Static-scale decode (M <= 8, FUSED): no quantiser launch.  Warp 8 quantises each k-block it hands to the MMA warps
-//     with the layer's s_in and fblk_code8, so the codes equal fp8ch_static_quant_kernel's.  Per-token scales depend on
-//     the whole row, which a split-K rank does not read: their decode runs fp8ch_quant_kernel and the GEMM under
+//     Static-scale decode (M <= 8, MODE 1 / 2): no quantiser launch.  Warp 8 quantises each k-block it hands to the MMA
+//     warps with the layer's s_in and fblk_code8, so the codes equal fp8ch_static_quant_kernel's.  Per-token scales
+//     depend on the whole row, which a split-K rank does not read: their decode runs fp8ch_quant_kernel and the GEMM under
 //     programmatic dependent launch, which measured faster than finding the row amax inside the GEMM (DESIGN.md).
+//   * int8ch_gemm_kernel: the same body (ch_gemm_body MODE 3) on m64nNk32.s32.s8.s8 into int32 registers that
+//     accumulate across all of the rank's k-blocks (integer sums are exact, so there is no per-block promotion), an
+//     integer DSMEM reduction, and float(acc) once in the same epilogue.  Both int8 activation kinds run a quantiser and
+//     the GEMM under programmatic dependent launch at every M.
 #include <cuda.h>
 
 #include <type_traits>
@@ -101,6 +108,56 @@ __global__ void __launch_bounds__(C_QUANT_THREADS)
   if (g < M) s_x[g] = s;
 }
 
+// eight int8 codes clamp(rint(x / s), -128, 127) (IEEE division, round half to even), packed in k order
+template <typename T>
+__device__ __forceinline__ uint2 int8_code8(const uint4& v, float s) {
+  const T* h = reinterpret_cast<const T*>(&v);
+  uint32_t w[2] = {0u, 0u};
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const float q = fminf(fmaxf(rintf(__fdiv_rn(ET<T>::to_f(h[e]), s)), -128.f), 127.f);
+    w[e >> 2] |= ((uint32_t)(int)q & 0xFFu) << (8 * (e & 3));
+  }
+  return make_uint2(w[0], w[1]);
+}
+
+// one CTA per token row m: s_x = max(amax, 1e-10) / 127; an all-zero row gets codes 0 and a finite scale
+template <typename T>
+__global__ void __launch_bounds__(C_QUANT_THREADS)
+    int8ch_quant_kernel(const T* __restrict__ x, int8_t* __restrict__ codes, float* __restrict__ s_x, int K) {
+  __shared__ float red[C_QUANT_THREADS / 32];
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // x is the previous kernel's output
+  const size_t row = (size_t)blockIdx.x * K;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row);
+  const int n8 = K / 8;
+  float a = 0.f;
+  for (int o = threadIdx.x; o < n8; o += C_QUANT_THREADS) a = fmaxf(a, amax8<T>(xr[o]));
+  a = warp_max(a);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = a;
+  __syncthreads();
+  a = 0.f;
+#pragma unroll
+  for (int w = 0; w < C_QUANT_THREADS / 32; ++w) a = fmaxf(a, red[w]);
+  const float s = fmaxf(a, 1e-10f) / 127.f;  // IEEE division
+  uint2* cr = reinterpret_cast<uint2*>(codes + row);
+  for (int o = threadIdx.x; o < n8; o += C_QUANT_THREADS) cr[o] = int8_code8<T>(xr[o], s);
+  if (threadIdx.x == 0) s_x[blockIdx.x] = s;
+}
+
+// elementwise over the M * K / 8 eight-element chunks; thread g < M also writes s_x[g] = s_in
+template <typename T>
+__global__ void __launch_bounds__(C_QUANT_THREADS)
+    int8ch_static_quant_kernel(const T* __restrict__ x, const float* __restrict__ s_in, int8_t* __restrict__ codes,
+                               float* __restrict__ s_x, int M, long long n8) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const long long g = (long long)blockIdx.x * C_QUANT_THREADS + threadIdx.x;
+  const float s = *s_in;
+  if (g < n8) reinterpret_cast<uint2*>(codes)[g] = int8_code8<T>(reinterpret_cast<const uint4*>(x)[g], s);
+  if (g < M) s_x[g] = s;
+}
+
 // ------------------------------------------------------------------------------------------------
 // GEMM
 // ------------------------------------------------------------------------------------------------
@@ -120,16 +177,17 @@ __device__ __forceinline__ void store_scaled4(T* dst, const float* __restrict__ 
   *reinterpret_cast<uint2*>(dst) = make_uint2(E::pack2(y[0], y[1]), E::pack2(y[2], y[3]));
 }
 
-// FUSED: 0 = codes and token scales come from a quantiser kernel (TMA for the codes); 1 / 2 = M <= 8, x fp16 / bf16 is
-// quantised by the producer with the static scale s_in
-template <int NTOK, int FUSED>
-__global__ void __launch_bounds__(C_THREADS, 1)
-    fp8ch_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
-                      const void* __restrict__ x, const float* __restrict__ s_x, const float* __restrict__ s_in,
-                      const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M, int K,
-                      int N, int kpc, int out_bf16) {
+// MODE: 0 = e4m3 codes and token scales come from a quantiser kernel (TMA for the codes); 1 / 2 = M <= 8, x fp16 / bf16
+// is quantised to e4m3 by the producer with the static scale s_in; 3 = int8 codes and token scales from a quantiser
+template <int NTOK, int MODE>
+__device__ __forceinline__ void ch_gemm_body(const CUtensorMap& tmap_w, const CUtensorMap& tmap_q,
+                                             const void* __restrict__ x, const float* __restrict__ s_x,
+                                             const float* __restrict__ s_in, const float* __restrict__ s_w,
+                                             const void* __restrict__ bias, void* __restrict__ out, int M, int K, int N,
+                                             int kpc, int out_bf16) {
   using C = FchCfg<NTOK>;
   constexpr int ST = C::ST;
+  constexpr bool FUSED = MODE == 1 || MODE == 2, S8 = MODE == 3;
   static_assert(!FUSED || NTOK == 8, "the fused quantiser serves 8-token tiles");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -180,8 +238,8 @@ __global__ void __launch_bounds__(C_THREADS, 1)
 
   if (warp == 8) {
     // ================================ producer ================================
-    if (FUSED) {
-      using T = typename std::conditional<FUSED == 1, __half, __nv_bfloat16>::type;
+    if constexpr (FUSED) {
+      using T = typename std::conditional<MODE == 1, __half, __nv_bfloat16>::type;
       // half-warp h of pass p holds token t = 2 p + h, lane j = lane & 15 its elements 8 j .. 8 j + 7 of the k-block;
       // rows t >= M keep the zero codes written here once
       constexpr int PD = 4;  // k-blocks of activations in flight ahead of the one being quantised
@@ -242,6 +300,29 @@ __global__ void __launch_bounds__(C_THREADS, 1)
         tma_load_2d(sX(s), &tmap_q, bar_full + 8 * s, (kb0 + i) * C_BK, row0);
       }
     }
+  } else if constexpr (S8) {
+    // ================================ MMA warpgroups, int8 ================================
+    // the int32 sums are exact (|acc| <= 2^30 for K <= 65536), so every k-block accumulates into the same registers
+    const int wg = warp >> 2;
+    int acc[C::ACC];
+#pragma unroll
+    for (int v = 0; v < C::ACC; ++v) acc[v] = 0;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % ST;
+      mbar_wait(bar_full + 8 * s, (i / ST) & 1);
+      const uint64_t wdesc = wgmma_desc_k_sw128(sW(s)) + 512 * wg;
+      const uint64_t xdesc = wgmma_desc_k_sw128(sX(s));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < C_BK / 32; ++k) Wgmma8<NTOK>::mma(acc, wdesc + 2 * k, xdesc + 2 * k, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+    }
+    asm volatile("bar.sync 1, %0;" ::"r"(C_MMA_THREADS) : "memory");
+    park_partial(smem_base, wg, warp & 3, acc);
   } else {
     // ================================ MMA warpgroups ================================
     const int wg = warp >> 2;  // features 64 wg .. 64 wg + 63 of the tile
@@ -277,7 +358,14 @@ __global__ void __launch_bounds__(C_THREADS, 1)
     if (nc < N) {
       for (int tok = (int)crank + (int)nrank * warp; tok < rows; tok += (int)nrank * (C_MMA_THREADS / 32)) {
         float a[1][4];
-        dsmem_sum4<1, false>(smem_base + (uint32_t)tok * (C_BF * 4) + (uint32_t)lane * 16, 0, nrank, a);
+        if constexpr (S8) {
+          int ia[1][4];
+          dsmem_sum4<1, true>(smem_base + (uint32_t)tok * (C_BF * 4) + (uint32_t)lane * 16, 0, nrank, ia);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) a[0][e] = __int2float_rn(ia[0][e]);  // one rounding of the exact sum
+        } else {
+          dsmem_sum4<1, false>(smem_base + (uint32_t)tok * (C_BF * 4) + (uint32_t)lane * 16, 0, nrank, a);
+        }
         const size_t o = (size_t)(row0 + tok) * N + nc;
         if (out_bf16)
           store_scaled4(reinterpret_cast<__nv_bfloat16*>(out) + o, s_w, reinterpret_cast<const __nv_bfloat16*>(bias),
@@ -290,6 +378,26 @@ __global__ void __launch_bounds__(C_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();  // keep every rank's shared memory alive until all peers have read it
+}
+
+// FUSED: 0 = e4m3 codes from a quantiser; 1 / 2 = static-scale decode of fp16 / bf16 x (MODE of ch_gemm_body)
+template <int NTOK, int FUSED>
+__global__ void __launch_bounds__(C_THREADS, 1)
+    fp8ch_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                      const void* __restrict__ x, const float* __restrict__ s_x, const float* __restrict__ s_in,
+                      const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M, int K,
+                      int N, int kpc, int out_bf16) {
+  ch_gemm_body<NTOK, FUSED>(tmap_w, tmap_q, x, s_x, s_in, s_w, bias, out, M, K, N, kpc, out_bf16);
+}
+
+// int8 codes from int8ch_quant_kernel / int8ch_static_quant_kernel and int8 weights
+template <int NTOK>
+__global__ void __launch_bounds__(C_THREADS, 1)
+    int8ch_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_q,
+                       const void* __restrict__ x, const float* __restrict__ s_x, const float* __restrict__ s_in,
+                       const float* __restrict__ s_w, const void* __restrict__ bias, void* __restrict__ out, int M,
+                       int K, int N, int kpc, int out_bf16) {
+  ch_gemm_body<NTOK, 3>(tmap_w, tmap_q, x, s_x, s_in, s_w, bias, out, M, K, N, kpc, out_bf16);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -315,20 +423,25 @@ int launch_fp8ch_static_quant(const void* x, const float* s_in, void* codes, flo
                        (const __nv_bfloat16*)x, s_in, (uint8_t*)codes, s_x, M, n8);
 }
 
-template <int NTOK, int FUSED>
+template <int NTOK, int MODE>
 static int launch_fp8ch_gemm_t(const Fp8ChArgs& a, const SwapPlan& p) {
   using C = FchCfg<NTOK>;
   CUtensorMap tw, tq;
   if (make_tmap_2d(&tw, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.weight, a.K, a.N, (size_t)a.K, C_BK, C_BF,
                    CU_TENSOR_MAP_SWIZZLE_128B) != 0)
     return -1;
-  if (FUSED) {
+  if (MODE == 1 || MODE == 2) {
     tq = tw;  // unused
   } else if (make_tmap_2d(&tq, CU_TENSOR_MAP_DATA_TYPE_UINT8, a.codes, a.K, a.M, (size_t)a.K, C_BK, NTOK,
                           CU_TENSOR_MAP_SWIZZLE_128B) != 0) {
     return -1;
   }
-  auto kern = fp8ch_gemm_kernel<NTOK, FUSED>;
+  void (*kern)(const CUtensorMap, const CUtensorMap, const void*, const float*, const float*, const float*, const void*,
+               void*, int, int, int, int, int);
+  if constexpr (MODE == 3)
+    kern = int8ch_gemm_kernel<NTOK>;
+  else
+    kern = fp8ch_gemm_kernel<NTOK, MODE>;
   static int smem_opted[32] = {};
   if (int e = ensure_dyn_smem(kern, C::SMEM_BYTES, smem_opted, "b2q_fp8ch")) return e;
   return launch_kernel(kern, dim3((a.N + C_BF - 1) / C_BF, p.ks, p.tblocks), dim3(C_THREADS, 1, 1), C::SMEM_BYTES,
@@ -346,6 +459,38 @@ int launch_fp8ch_gemm(const Fp8ChArgs& a) {
     case 32: return launch_fp8ch_gemm_t<32, 0>(a, p);
     case 64: return launch_fp8ch_gemm_t<64, 0>(a, p);
     default: return launch_fp8ch_gemm_t<128, 0>(a, p);
+  }
+}
+
+int launch_int8ch_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream) {
+  const dim3 grid((unsigned)M, 1, 1), block(C_QUANT_THREADS, 1, 1);
+  if (dtype == 0)
+    return launch_kernel(int8ch_quant_kernel<__half>, grid, block, 0, stream, 0, true, (const __half*)x, (int8_t*)codes,
+                         s_x, K);
+  return launch_kernel(int8ch_quant_kernel<__nv_bfloat16>, grid, block, 0, stream, 0, true, (const __nv_bfloat16*)x,
+                       (int8_t*)codes, s_x, K);
+}
+
+int launch_int8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                               cudaStream_t stream) {
+  const long long n8 = (long long)M * (K / 8), threads = n8 > M ? n8 : M;
+  const dim3 grid((unsigned)((threads + C_QUANT_THREADS - 1) / C_QUANT_THREADS), 1, 1), block(C_QUANT_THREADS, 1, 1);
+  if (dtype == 0)
+    return launch_kernel(int8ch_static_quant_kernel<__half>, grid, block, 0, stream, 0, true, (const __half*)x, s_in,
+                         (int8_t*)codes, s_x, M, n8);
+  return launch_kernel(int8ch_static_quant_kernel<__nv_bfloat16>, grid, block, 0, stream, 0, true,
+                       (const __nv_bfloat16*)x, s_in, (int8_t*)codes, s_x, M, n8);
+}
+
+// int8 codes (a.x == nullptr): the plan and tiles of the e4m3 GEMM
+int launch_int8ch_gemm(const Fp8ChArgs& a) {
+  const SwapPlan p = fp8blk_plan(0, a.M, a.K, a.N, 1, a.ks);
+  switch (p.ntok) {
+    case 8: return launch_fp8ch_gemm_t<8, 3>(a, p);
+    case 16: return launch_fp8ch_gemm_t<16, 3>(a, p);
+    case 32: return launch_fp8ch_gemm_t<32, 3>(a, p);
+    case 64: return launch_fp8ch_gemm_t<64, 3>(a, p);
+    default: return launch_fp8ch_gemm_t<128, 3>(a, p);
   }
 }
 

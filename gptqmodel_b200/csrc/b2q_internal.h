@@ -128,6 +128,11 @@ int launch_fp8ch_quant(const void* x, void* codes, float* s_x, int M, int K, flo
 int launch_fp8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
                               cudaStream_t stream);
 int launch_fp8ch_gemm(const Fp8ChArgs& a);
+// int8 W8A8 (compressed-tensors int-quantized) on the same GEMM: int8 codes and weights, Fp8ChArgs with x == nullptr
+int launch_int8ch_quant(const void* x, void* codes, float* s_x, int M, int K, int dtype, cudaStream_t stream);
+int launch_int8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                               cudaStream_t stream);
+int launch_int8ch_gemm(const Fp8ChArgs& a);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

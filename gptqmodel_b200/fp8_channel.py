@@ -33,13 +33,14 @@ def channel_scales(weight_scale: torch.Tensor, out_features: int) -> torch.Tenso
     return weight_scale.to(torch.float32).reshape(-1).expand(out_features).contiguous()
 
 
-class B200ChannelFp8Linear(nn.Module):
-    """Per-channel / per-tensor FP8 linear (buffers ``weight``, ``weight_scale``, ``input_scale``, ``bias``) on the
-    sm_90a e4m3 wgmma kernels.  ``activation``: "dynamic" (per-token scales, optionally bounded by ``ub``) or
-    "static" (the per-tensor ``input_scale``)."""
+class ChannelW8A8Linear(nn.Module):
+    """The module contract shared by the per-channel 8-bit W8A8 layers (buffers ``weight`` [N, K] of CODE_DTYPE codes,
+    ``weight_scale``, ``input_scale``, ``bias``).  A subclass names its code dtype and runs its forward ABI call."""
+
+    CODE_DTYPE: torch.dtype       # the weight codes the kernels read
+    WEIGHT_DTYPES: tuple = ()     # checkpoint weight dtypes accepted (viewed as CODE_DTYPE)
 
     SUPPORTS_BACKENDS = ["b200"]
-    SUPPORTS_METHODS = ["compressed-tensors", "fbgemm_fp8"]
     SUPPORTS_BITS = [8]
     SUPPORTS_SHARDS = False
     SUPPORTS_TRAINING = False
@@ -50,7 +51,6 @@ class B200ChannelFp8Linear(nn.Module):
     SUPPORTS_DEVICES = ["cuda"]
     SUPPORTS_PLATFORM = ["linux"]
     SUPPORTS_DTYPES = [torch.float16, torch.bfloat16]
-    QUANT_TYPE = "b200_fp8_channel"
 
     def __init__(self, in_features: int, out_features: int, bias: bool = False, activation: str = "dynamic",
                  ub: Optional[float] = None, adapter=None, register_buffers: bool = True, **kwargs):
@@ -68,7 +68,7 @@ class B200ChannelFp8Linear(nn.Module):
         self.name = kwargs.get("name") or f"{self.__class__.__module__}.{self.__class__.__qualname__}"
         self.adapter = adapter
         if register_buffers:
-            self.register_buffer("weight", torch.zeros((out_features, in_features), dtype=torch.float8_e4m3fn))
+            self.register_buffer("weight", torch.zeros((out_features, in_features), dtype=self.CODE_DTYPE))
             self.register_buffer("weight_scale", torch.ones((out_features, 1), dtype=torch.float32))
             if activation == "static":
                 self.register_buffer("input_scale", torch.ones(1, dtype=torch.float32))
@@ -97,8 +97,9 @@ class B200ChannelFp8Linear(nn.Module):
     def check_tensors(self) -> None:
         """dtype, shape and values of the checkpoint tensors; ValueError / NotImplementedError when they do not fit."""
         K, N = self.in_features, self.out_features
-        if self.weight.dtype not in (torch.float8_e4m3fn, torch.uint8):
-            raise NotImplementedError(f"{self.name}: weight dtype {self.weight.dtype} is not float8_e4m3fn")
+        if self.weight.dtype not in self.WEIGHT_DTYPES:
+            raise NotImplementedError(f"{self.name}: weight dtype {self.weight.dtype} is not "
+                                      f"{str(self.CODE_DTYPE).replace('torch.', '')}")
         if tuple(self.weight.shape) != (N, K):
             raise ValueError(f"{self.name}: weight {tuple(self.weight.shape)} is not [{N}, {K}]")
         ws = self.weight_scale
@@ -133,7 +134,7 @@ class B200ChannelFp8Linear(nn.Module):
         self.check_tensors()
         N = self.out_features
         self.scale_dtype = self.weight_scale.dtype
-        self.weight = _aligned(self.weight.data.view(torch.float8_e4m3fn))
+        self.weight = _aligned(self.weight.data.view(self.CODE_DTYPE))
         self.weight_scale = _aligned(channel_scales(self.weight_scale.data.to(dev), N))
         if self.input_scale is not None:
             self.input_scale = _aligned(self.input_scale.data.to(device=dev, dtype=torch.float32).reshape(1))
@@ -161,13 +162,7 @@ class B200ChannelFp8Linear(nn.Module):
         M = x2.shape[0]
         out = torch.empty((M, N), dtype=x.dtype, device=x.device)
         if M > 0:
-            nws = int(lib.b2q_fp8ch_workspace_bytes(M, K))
-            ws = torch.empty(nws, dtype=torch.uint8, device=x.device) if nws else None
-            ub = float("inf") if self.ub is None else self.ub
-            check(lib.b2q_fp8ch_forward(_ptr(x2), _ptr(self.weight), _ptr(self.weight_scale), _ptr(self.input_scale),
-                                        ub, _ptr(self._bias.get(x.dtype)), _ptr(out), M, K, N, _DTYPE_CODE[x.dtype],
-                                        _ptr(ws), nws, torch.cuda.current_stream(x.device).cuda_stream),
-                  "b2q_fp8ch_forward")
+            self._launch(x2, out)
         if self.adapter:
             out = self.adapter.apply(x=x2, out=out)
         return out.reshape(out_shape)
@@ -181,7 +176,7 @@ class B200ChannelFp8Linear(nn.Module):
         if dtype not in _DTYPE_CODE:
             raise NotImplementedError(f"{self.name}: dequantize_weight() computes fp16 or bf16 weights, not {dtype}")
         sd = self.scale_dtype if self._ready else self.weight_scale.dtype
-        w = self.weight.view(torch.float8_e4m3fn)
+        w = self.weight.view(self.CODE_DTYPE)
         s = self.weight_scale.to(device=w.device, dtype=sd).reshape(-1)
         s = s[:, None] if s.numel() > 1 else s.reshape(())
         out = (w.to(sd) * s).to(dtype).t().contiguous()
@@ -207,6 +202,27 @@ class B200ChannelFp8Linear(nn.Module):
         if post_init:
             m.post_init()
         return m
+
+
+class B200ChannelFp8Linear(ChannelW8A8Linear):
+    """Per-channel / per-tensor FP8 linear (buffers ``weight``, ``weight_scale``, ``input_scale``, ``bias``) on the
+    sm_90a e4m3 wgmma kernels.  ``activation``: "dynamic" (per-token scales, optionally bounded by ``ub``) or
+    "static" (the per-tensor ``input_scale``)."""
+
+    CODE_DTYPE = torch.float8_e4m3fn
+    WEIGHT_DTYPES = (torch.float8_e4m3fn, torch.uint8)
+    SUPPORTS_METHODS = ["compressed-tensors", "fbgemm_fp8"]
+    QUANT_TYPE = "b200_fp8_channel"
+
+    def _launch(self, x2: torch.Tensor, out: torch.Tensor) -> None:
+        (M, K), N = x2.shape, self.out_features
+        nws = int(lib.b2q_fp8ch_workspace_bytes(M, K))
+        ws = torch.empty(nws, dtype=torch.uint8, device=x2.device) if nws else None
+        ub = float("inf") if self.ub is None else self.ub
+        check(lib.b2q_fp8ch_forward(_ptr(x2), _ptr(self.weight), _ptr(self.weight_scale), _ptr(self.input_scale),
+                                    ub, _ptr(self._bias.get(x2.dtype)), _ptr(out), M, K, N, _DTYPE_CODE[x2.dtype],
+                                    _ptr(ws), nws, torch.cuda.current_stream(x2.device).cuda_stream),
+              "b2q_fp8ch_forward")
 
     def extra_repr(self) -> str:
         act = "static per-tensor" if self.activation == "static" else "dynamic per-token"

@@ -329,10 +329,15 @@ class Fp8W8A8Spec:
     def ignores(self, name: str) -> bool:
         if self.method == "fbgemm_fp8":  # transformers' modules_to_not_convert: a fragment of the module's name
             return any(k in name for k in self.ignore)
-        return any(re.match(k[3:], name) if k.startswith("re:") else k == name for k in self.ignore)
+        return _ct_ignores(self.ignore, name)
 
 
-def _ct_args(where: str, a, kinds) -> tuple:
+def _ct_ignores(ignore: tuple, name: str) -> bool:
+    """compressed-tensors `ignore`: module names and `re:` patterns."""
+    return any(re.match(k[3:], name) if k.startswith("re:") else k == name for k in ignore)
+
+
+def _ct_args(where: str, a, kinds, want: str = "float") -> tuple:
     """(strategy, dynamic) of one compressed-tensors QuantizationArgs dict that this package serves."""
     if not isinstance(a, dict):
         raise ValueError(f"compressed-tensors: `{where}` must be a dict, got {a!r}")
@@ -343,8 +348,8 @@ def _ct_args(where: str, a, kinds) -> tuple:
         raise ValueError(f"compressed-tensors: `{where}` needs type int | float, a boolean `symmetric` and a `strategy`")
     if not (isinstance(dyn, bool) or dyn == "local"):
         raise ValueError(f"compressed-tensors: `{where}.dynamic` must be a boolean, got {dyn!r}")
-    if typ != "float" or nb != 8:
-        raise NotImplementedError(f"compressed-tensors: {where} of {nb}-bit {typ} are not served (8-bit float only)")
+    if typ != want or nb != 8:
+        raise NotImplementedError(f"compressed-tensors: {where} of {nb}-bit {typ} are not served (8-bit {want} only)")
     if not sym:
         raise NotImplementedError(f"compressed-tensors: asymmetric {where} are not served")
     if strat not in ("tensor", "channel", "group", "block", "token", "tensor_group", "attn_head"):
@@ -353,6 +358,53 @@ def _ct_args(where: str, a, kinds) -> tuple:
         raise NotImplementedError(f"compressed-tensors: {where} with strategy `{strat}`, dynamic={dyn} are not served "
                                   f"(served: {', '.join(f'{s} / dynamic={d}' for s, d in kinds)})")
     return strat, dyn
+
+
+def _ct_w8a8(raw: dict, fmt_name: str, want: str) -> tuple:
+    """(weight strategy, activation kind, ignore, kv_cache_scheme) of a compressed-tensors W8A8 config whose groups all
+    target ["Linear"] with 8-bit `want` (float | int) symmetric weights (channel | tensor, static) and input activations
+    (token / dynamic or tensor / static), the same kind in every group."""
+    fmt = raw.get("format")
+    if fmt != fmt_name:
+        raise NotImplementedError(f"compressed-tensors: format `{fmt}` is not served ({fmt_name} only)")
+    groups = raw.get("config_groups")
+    if not isinstance(groups, dict) or not groups:
+        raise ValueError("compressed-tensors: `config_groups` must be a non-empty dict")
+    kinds = set()
+    for gname, g in groups.items():
+        if not isinstance(g, dict):
+            raise ValueError(f"compressed-tensors: config group `{gname}` must be a dict")
+        targets = g.get("targets")
+        if not (isinstance(targets, list) and all(isinstance(t, str) for t in targets)):
+            raise ValueError(f"compressed-tensors: `{gname}.targets` must be a list of names")
+        if targets != ["Linear"]:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` targets {targets} (only [\"Linear\"] is served)")
+        if g.get("format") not in (None, fmt_name):
+            raise NotImplementedError(f"compressed-tensors: `{gname}` has format `{g.get('format')}`")
+        if g.get("output_activations") is not None:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` quantises output activations")
+        if g.get("weights") is None or g.get("input_activations") is None:
+            raise NotImplementedError(f"compressed-tensors: `{gname}` is not W8A8 (weights and input activations)")
+        ws, _ = _ct_args(f"{gname}.weights", g["weights"], {("channel", False), ("tensor", False)}, want)
+        _, dyn = _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True), ("tensor", False)},
+                           want)
+        kinds.add((ws, "dynamic" if dyn else "static"))
+    if len(kinds) != 1:
+        raise NotImplementedError(f"compressed-tensors: mixed config groups {sorted(kinds)} are not served")
+    ignore = raw.get("ignore") or []
+    if not (isinstance(ignore, (list, tuple)) and all(isinstance(s, str) for s in ignore)):
+        raise ValueError(f"compressed-tensors: `ignore` must be a list of names, got {ignore!r}")
+    for k in ignore:
+        if k.startswith("re:"):
+            try:
+                re.compile(k[3:])
+            except re.error as e:
+                raise ValueError(f"compressed-tensors: bad `ignore` pattern `{k}`: {e}") from None
+    kv = raw.get("kv_cache_scheme")
+    if kv is not None and not isinstance(kv, dict):
+        raise ValueError(f"compressed-tensors: `kv_cache_scheme` must be a dict, got {kv!r}")
+    (ws, act), = kinds
+    return ws, act, tuple(ignore), kv
 
 
 def parse_fp8_w8a8_config(raw: dict) -> Fp8W8A8Spec:
@@ -377,46 +429,8 @@ def parse_fp8_w8a8_config(raw: dict) -> Fp8W8A8Spec:
         return Fp8W8A8Spec("fbgemm_fp8", "channel", "dynamic", float(ub), tuple(skip))
     if method != "compressed-tensors":
         raise NotImplementedError(f"FP8 W8A8: quant_method `{method}` is not compressed-tensors or fbgemm_fp8")
-    fmt = raw.get("format")
-    if fmt != "float-quantized":
-        raise NotImplementedError(f"compressed-tensors: format `{fmt}` is not served (float-quantized only)")
-    groups = raw.get("config_groups")
-    if not isinstance(groups, dict) or not groups:
-        raise ValueError("compressed-tensors: `config_groups` must be a non-empty dict")
-    kinds = set()
-    for gname, g in groups.items():
-        if not isinstance(g, dict):
-            raise ValueError(f"compressed-tensors: config group `{gname}` must be a dict")
-        targets = g.get("targets")
-        if not (isinstance(targets, list) and all(isinstance(t, str) for t in targets)):
-            raise ValueError(f"compressed-tensors: `{gname}.targets` must be a list of names")
-        if targets != ["Linear"]:
-            raise NotImplementedError(f"compressed-tensors: `{gname}` targets {targets} (only [\"Linear\"] is served)")
-        if g.get("format") not in (None, "float-quantized"):
-            raise NotImplementedError(f"compressed-tensors: `{gname}` has format `{g.get('format')}`")
-        if g.get("output_activations") is not None:
-            raise NotImplementedError(f"compressed-tensors: `{gname}` quantises output activations")
-        if g.get("weights") is None or g.get("input_activations") is None:
-            raise NotImplementedError(f"compressed-tensors: `{gname}` is not W8A8 (weights and input activations)")
-        ws, _ = _ct_args(f"{gname}.weights", g["weights"], {("channel", False), ("tensor", False)})
-        _, dyn = _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True), ("tensor", False)})
-        kinds.add((ws, "dynamic" if dyn else "static"))
-    if len(kinds) != 1:
-        raise NotImplementedError(f"compressed-tensors: mixed config groups {sorted(kinds)} are not served")
-    ignore = raw.get("ignore") or []
-    if not (isinstance(ignore, (list, tuple)) and all(isinstance(s, str) for s in ignore)):
-        raise ValueError(f"compressed-tensors: `ignore` must be a list of names, got {ignore!r}")
-    for k in ignore:
-        if k.startswith("re:"):
-            try:
-                re.compile(k[3:])
-            except re.error as e:
-                raise ValueError(f"compressed-tensors: bad `ignore` pattern `{k}`: {e}") from None
-    kv = raw.get("kv_cache_scheme")
-    if kv is not None and not isinstance(kv, dict):
-        raise ValueError(f"compressed-tensors: `kv_cache_scheme` must be a dict, got {kv!r}")
-    (ws, act), = kinds
-    return Fp8W8A8Spec("compressed-tensors", ws, act, None, tuple(ignore), kv)
+    ws, act, ignore, kv = _ct_w8a8(raw, "float-quantized", "float")
+    return Fp8W8A8Spec("compressed-tensors", ws, act, None, ignore, kv)
 
 
 @torch.no_grad()
@@ -432,11 +446,19 @@ def load_fp8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype]
     only      : optional iterable of module prefixes to load (default: all found)
     post_init : default True on CUDA devices, False on CPU (tensors only; host tests)
     """
-    from safetensors import safe_open
-
     from .fp8_channel import B200ChannelFp8Linear
 
     spec = parse_fp8_w8a8_config(_read_raw_config(path))
+    return _load_channel_w8a8(path, spec, B200ChannelFp8Linear, device, dtype, only, post_init)
+
+
+def _load_channel_w8a8(path: str, spec, cls, device, dtype, only, post_init) -> Dict[str, nn.Module]:
+    """The `<prefix>.weight` + `<prefix>.weight_scale` modules of a per-channel W8A8 checkpoint as `cls` modules (their
+    weights of cls.CODE_DTYPE).  A `weight_zero_point` / `input_zero_point` tensor must be all zeros: the kernels are
+    symmetric."""
+    from safetensors import safe_open
+
+    code = str(cls.CODE_DTYPE).replace("torch.", "")
     wmap = _weight_map(path)
     if only is not None:
         prefixes = list(only)
@@ -462,9 +484,13 @@ def load_fp8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype]
             t = {s: tensor(f"{prefix}.{s}") for s in ("weight", "weight_scale", "input_scale", "bias")}
             if t["weight"] is None or t["weight_scale"] is None:
                 raise KeyError(f"{prefix}: checkpoint misses weight / weight_scale")
-            if t["weight"].dtype != torch.float8_e4m3fn:
+            if t["weight"].dtype != cls.CODE_DTYPE:
                 raise NotImplementedError(f"{prefix}: weight dtype {t['weight'].dtype} is not served "
-                                          "(float8_e4m3fn only)")
+                                          f"({code} only)")
+            for zp in ("weight_zero_point", "input_zero_point"):
+                z = tensor(f"{prefix}.{zp}")
+                if z is not None and bool((z.to(torch.float32) != 0).any()):
+                    raise NotImplementedError(f"{prefix}: a non-zero `{zp}` (asymmetric quantisation) is not served")
             if spec.activation == "static" and t["input_scale"] is None:
                 raise NotImplementedError(f"{prefix}: static activations need `input_scale`, the checkpoint has none")
             if spec.activation == "dynamic" and t["input_scale"] is not None:
@@ -472,7 +498,7 @@ def load_fp8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype]
             ws = t["weight_scale"]
             if spec.weight_strategy == "tensor" and ws.numel() != 1:
                 raise ValueError(f"{prefix}: per-tensor weight_scale has shape {tuple(ws.shape)}")
-            mods[prefix] = B200ChannelFp8Linear.from_checkpoint_tensors(
+            mods[prefix] = cls.from_checkpoint_tensors(
                 t["weight"], ws, input_scale=t["input_scale"], bias=t["bias"], activation=spec.activation,
                 ub=spec.ub, device=dev, dtype=dtype, post_init=do_post, name=prefix)
     finally:
@@ -482,6 +508,53 @@ def load_fp8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype]
                 close(None, None, None)
         handles.clear()
     return mods
+
+
+@dataclass
+class Int8W8A8Spec:
+    """A per-channel / per-tensor INT8 (W8A8) config: compressed-tensors `int-quantized`.  kv_cache_scheme is returned
+    untouched, as for Fp8W8A8Spec."""
+    weight_strategy: str = "channel"  # "channel" | "tensor"
+    activation: str = "dynamic"       # "dynamic" (per token) | "static" (per tensor, input_scale)
+    ignore: tuple = ()                # names / "re:" patterns
+    kv_cache_scheme: Optional[dict] = None
+    ub = None                         # int8 activations have no amax bound
+
+    def ignores(self, name: str) -> bool:
+        return _ct_ignores(self.ignore, name)
+
+
+def parse_int8_w8a8_config(raw: dict) -> Int8W8A8Spec:
+    """Per-channel / per-tensor INT8 (W8A8) configs: `quant_method: compressed-tensors`, `format: int-quantized`; every
+    config group targets ["Linear"] with weights {num_bits: 8, type: int, symmetric: true, dynamic: false, strategy:
+    channel | tensor} and input activations {num_bits: 8, type: int, symmetric: true} either {strategy: token, dynamic:
+    true} or {strategy: tensor, dynamic: false}, the same in every group.  `ignore` holds module names and `re:`
+    patterns.  NotImplementedError for what the kernels do not serve (asymmetric activations, group / block strategies,
+    float or 4-bit types, pack-quantized, mixed groups, output activations, other targets), ValueError for malformed
+    entries."""
+    if not isinstance(raw, dict):
+        raise ValueError(f"INT8 W8A8: the quantisation config must be a dict, got {type(raw).__name__}")
+    method = raw.get("quant_method")
+    if method != "compressed-tensors":
+        raise NotImplementedError(f"INT8 W8A8: quant_method `{method}` is not compressed-tensors")
+    ws, act, ignore, kv = _ct_w8a8(raw, "int-quantized", "int")
+    return Int8W8A8Spec(ws, act, ignore, kv)
+
+
+@torch.no_grad()
+def load_int8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype] = None,
+                           only: Optional[Iterable[str]] = None,
+                           post_init: Optional[bool] = None) -> Dict[str, nn.Module]:
+    """Load every INT8 W8A8 linear of a compressed-tensors `int-quantized` checkpoint into B200ChannelInt8Linear
+    modules, as load_fp8_w8a8_linears does for FP8: ignored modules stay dense and are not returned, a static layer must
+    carry its `input_scale` and a dynamic one must not, and zero-point tensors must be all zeros (NotImplementedError).
+    only      : optional iterable of module prefixes to load (default: all found)
+    post_init : default True on CUDA devices, False on CPU (tensors only; host tests)
+    """
+    from .int8_channel import B200ChannelInt8Linear
+
+    spec = parse_int8_w8a8_config(_read_raw_config(path))
+    return _load_channel_w8a8(path, spec, B200ChannelInt8Linear, device, dtype, only, post_init)
 
 
 def _weight_map(path: str) -> Dict[str, str]:

@@ -379,6 +379,40 @@ int b2q_fp8ch_forward(const void* x, const void* weight, const float* s_w, const
                       const void* bias, void* out, int M, int K, int N, int dtype, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* Per-channel INT8 (W8A8) layers (an addition to ABI v8 that changes no earlier entry point): compressed-tensors
+ * `int-quantized` W8A8 (channel or tensor weights; dynamic per-token or static per-tensor activations).  Weights int8
+ * w [N, K] (the checkpoint tensor, unchanged), s_w fp32 [N] as for per-channel FP8.  T = fp16 (dtype 0) or bf16
+ * (dtype 1).  For every token row m:
+ *   dynamic: s_x[m] = fmaxf(max_k |x[m,k]|, 1e-10f) / 127.f                   (IEEE fp32 division)
+ *   static:  s_x[m] = s_in                                                    (the layer's input_scale)
+ *   q[m,k]   = (int8) clamp(rint(float(x[m,k]) / s_x[m]), -128, 127)         (IEEE fp32 division, half to even)
+ *   acc[m,n] = sum_k q[m,k] * w[n,k]                                          (int32, exact: |acc| <= 2^30)
+ *   y        = T(__fmul_rn(float(acc), __fmul_rn(s_x[m], s_w[n])) + bias[n])  (float(acc) rounds to nearest; fp32
+ *                                                                              products and sum, NOT fused; one
+ *                                                                              rounding to T; bias optional, T [N])
+ * An all-zero row gets codes 0 and a finite scale.  The sum is exact, so the output does not depend on the split-K
+ * plan: ks = 1, 2, ... and the heuristic give the same bits.  The s8 wgmma accumulates every k-block into the same int32
+ * registers and the ranks' partials are added as integers over distributed shared memory.  The envelope is that of
+ * per-channel FP8 (K % 128 == 0, K <= 65536, N % 64 == 0; 16-byte aligned x, codes, weight, s_w, out, workspace and
+ * the quantisers' s_x).  Bad arguments return -2 before any CUDA work. */
+/* Workspace of b2q_int8ch_forward for M rows: the codes and token scales. */
+size_t b2q_int8ch_workspace_bytes(int M, int K);
+/* Dynamic per-token quantiser: x T [M, K] -> codes int8 [M, K], s_x fp32 [M]; programmatic dependent launch. */
+int b2q_int8ch_quantize(const void* x, void* codes, float* s_x, int M, int K, int dtype, void* stream);
+/* Static quantiser: codes of x / s_in with s_in a device fp32 [1]; s_x[m] = s_in for every row. */
+int b2q_int8ch_quantize_static(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
+                               void* stream);
+/* out T [M, N] from either quantiser's codes and scales; ks = split-K ranks (1..8), <= 0: the heuristic (the plan of
+ * b2q_fp8ch_mm). */
+int b2q_int8ch_mm(const void* codes, const float* s_x, const void* weight, const float* s_w, const void* bias, void* out,
+                  int M, int K, int N, int dtype, int ks, void* stream);
+/* The layer: s_in != NULL selects static scales, else dynamic per-token scales.  A quantiser + b2q_int8ch_mm (ks <= 0)
+ * through the workspace under programmatic dependent launch at every M, so the output is identical to theirs.
+ * Dispatches on M inside the library, so a CUDA graph sees the true M. */
+int b2q_int8ch_forward(const void* x, const void* weight, const float* s_w, const float* s_in, const void* bias,
+                       void* out, int M, int K, int N, int dtype, void* workspace, size_t workspace_bytes,
+                       void* stream);
+
 /* Block-FP8 MoE experts (an addition to ABI v8): the experts' w1 / w3 [E*I, K], w2 [E*H, I] e4m3 stacks and their scale
  * stacks [E, ceil(N/128), K/128] (each expert's checkpoint tensors, back to back), the routing tables of b2q_moe_align.
  * One block is six launches with no host synchronisation: b2q_moe_align, b2q_fp8blk_moe_gather, b2q_fp8blk_moe_gate_up,
