@@ -76,6 +76,12 @@ SYMBOLS = {
     "b2q_qqq_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8ch_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
+    "b2q_fp8ch_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_fp8ch_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_int8ch_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b2q_int8ch_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b2q_int8ch_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

@@ -1012,6 +1012,112 @@ int b2q_fp8blk_moe_down(const void* codes_h, const float* s_h, const void* w2, c
   return check_cuda(launch_fp8blk_moe(2, a, g), "b2q_fp8blk_moe_down");
 }
 
+// ---- per-channel W8A8 MoE experts (FP8 and INT8): the grouped modes of the b2q_fp8ch GEMM over b2q_moe_align's tables ----
+static int ch_moe_gather(const char* fn, int s8, const void* x, const int32_t* sorted_pairs, const int32_t* offsets,
+                         const float* s_in, int E, void* codes, float* s_x, int T, int top_k, int K, float ub, int dtype,
+                         void* stream) {
+  if (T < 1 || top_k < 1) {
+    set_error("%s: T=%d, top_k=%d must be >= 1", fn, T, top_k);
+    return -2;
+  }
+  if (int e = fp8blk_check_shape(fn, T * top_k, K, 64, dtype)) return e;
+  if (!s8 && s_in == nullptr) {
+    if (int e = fp8ch_check_ub(fn, ub)) return e;
+  }
+  if (x == nullptr || codes == nullptr || s_x == nullptr || !aligned16(x) || !aligned16(codes) || !aligned16(s_x)) {
+    set_error("%s: x, codes and s_x must be 16-byte aligned device pointers", fn);
+    return -2;
+  }
+  if (s_in != nullptr && (offsets == nullptr || E < 1 || E > 256)) {
+    set_error("%s: static scales need the offsets of b2q_moe_align and E=%d in 1..256", fn, E);
+    return -2;
+  }
+  DeviceGuard dg(codes);
+  return check_cuda(launch_ch_moe_gather(s8, x, sorted_pairs, offsets, s_in, E, codes, s_x, T * top_k, top_k, K, ub,
+                                         dtype, (cudaStream_t)stream),
+                    fn);
+}
+
+static int ch_moe_gate_up(const char* fn, int s8, const void* codes, const float* s_x, const void* w1,
+                          const float* s_w1, const void* w3, const float* s_w3, void* h, const int32_t* counts,
+                          const int32_t* offsets, int E, int rows, int active, int K, int N, int dtype, int ks,
+                          void* stream) {
+  if (int e = fp8blk_moe_check(fn, codes, s_x, w1, s_w1, h, counts, offsets, E, rows, K, N, dtype, ks)) return e;
+  if (int e = fp8blk_check_layer(fn, w3, s_w3, h)) return e;
+  DeviceGuard dg(w1);
+  Fp8ChArgs a = {nullptr, codes, s_x, nullptr, w1, s_w1, nullptr, h, rows, K, N, dtype, ks, (cudaStream_t)stream};
+  Fp8ChMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.w3 = w3;
+  g.s_w3 = s_w3;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_ch_moe(1, s8, a, g), fn);
+}
+
+static int ch_moe_down(const char* fn, int s8, const void* codes_h, const float* s_h, const void* w2, const float* s_w2,
+                       const int32_t* counts, const int32_t* offsets, const int32_t* sorted_pairs,
+                       const float* pair_weights, float* ypair, int E, int rows, int active, int K, int N, int dtype,
+                       int ks, void* stream) {
+  if (int e = fp8blk_moe_check(fn, codes_h, s_h, w2, s_w2, ypair, counts, offsets, E, rows, K, N, dtype, ks)) return e;
+  if (sorted_pairs == nullptr || pair_weights == nullptr) {
+    set_error("%s: sorted_pairs and pair_weights must be device pointers", fn);
+    return -2;
+  }
+  DeviceGuard dg(w2);
+  Fp8ChArgs a = {nullptr, codes_h, s_h, nullptr, w2, s_w2, nullptr, ypair, rows, K, N, dtype, ks, (cudaStream_t)stream};
+  Fp8ChMoe g = {};
+  g.counts = counts;
+  g.offsets = offsets;
+  g.sorted_pairs = sorted_pairs;
+  g.pair_weights = pair_weights;
+  g.ypair = ypair;
+  g.E = E;
+  g.active = active;
+  return check_cuda(launch_ch_moe(2, s8, a, g), fn);
+}
+
+int b2q_fp8ch_moe_gather(const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in, int E,
+                         void* codes, float* s_x, int T, int top_k, int K, float ub, int dtype, void* stream) {
+  return ch_moe_gather("b2q_fp8ch_moe_gather", 0, x, sorted_pairs, offsets, s_in, E, codes, s_x, T, top_k, K, ub, dtype,
+                       stream);
+}
+
+int b2q_fp8ch_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                          const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                          int active, int K, int N, int dtype, int ks, void* stream) {
+  return ch_moe_gate_up("b2q_fp8ch_moe_gate_up", 0, codes, s_x, w1, s_w1, w3, s_w3, h, counts, offsets, E, rows, active,
+                        K, N, dtype, ks, stream);
+}
+
+int b2q_fp8ch_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                       const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                       int E, int rows, int active, int K, int N, int dtype, int ks, void* stream) {
+  return ch_moe_down("b2q_fp8ch_moe_down", 0, codes_h, s_h, w2, s_w2, counts, offsets, sorted_pairs, pair_weights, ypair,
+                     E, rows, active, K, N, dtype, ks, stream);
+}
+
+int b2q_int8ch_moe_gather(const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in, int E,
+                          void* codes, float* s_x, int T, int top_k, int K, int dtype, void* stream) {
+  return ch_moe_gather("b2q_int8ch_moe_gather", 1, x, sorted_pairs, offsets, s_in, E, codes, s_x, T, top_k, K, 0.f,
+                       dtype, stream);
+}
+
+int b2q_int8ch_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                           const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                           int active, int K, int N, int dtype, int ks, void* stream) {
+  return ch_moe_gate_up("b2q_int8ch_moe_gate_up", 1, codes, s_x, w1, s_w1, w3, s_w3, h, counts, offsets, E, rows,
+                        active, K, N, dtype, ks, stream);
+}
+
+int b2q_int8ch_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                        const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                        int E, int rows, int active, int K, int N, int dtype, int ks, void* stream) {
+  return ch_moe_down("b2q_int8ch_moe_down", 1, codes_h, s_h, w2, s_w2, counts, offsets, sorted_pairs, pair_weights,
+                     ypair, E, rows, active, K, N, dtype, ks, stream);
+}
+
 int b2q_gemv(const void* x, const void* packed, const void* scales, const int32_t* qzeros, const int32_t* perm,
              const void* bias, void* out, int K, int N, int bits, int group_size, int dtype, int ks, int warps,
              void* stream) {

@@ -133,6 +133,25 @@ int launch_int8ch_quant(const void* x, void* codes, float* s_x, int M, int K, in
 int launch_int8ch_static_quant(const void* x, const float* s_in, void* codes, float* s_x, int M, int K, int dtype,
                                cudaStream_t stream);
 int launch_int8ch_gemm(const Fp8ChArgs& a);
+// grouped (MoE) launches of the per-channel W8A8 GEMM (s8 = 1: int8, 0: e4m3): a = {codes / s_x = the expert-sorted
+// rows [M = rows, K] / [rows], weight / s_w = the stacked w1 (mode 1) or w2 (mode 2) [E*N, K] / [E, N], out = h
+// [rows, N] (mode 1), N / K of ONE expert, ks <= 0: heuristic}
+struct Fp8ChMoe {
+  const int32_t* counts;        // [E]
+  const int32_t* offsets;       // [E]
+  const int32_t* sorted_pairs;  // [rows]     (mode 2)
+  const float* pair_weights;    // [rows]     (mode 2)
+  const void* w3;               // mode 1: the up stack, shaped like the gate stack
+  const float* s_w3;
+  float* ypair;                 // mode 2: [rows, N] fp32
+  int E, active;                // experts, experts expected to be active (grid sizing only)
+};
+int launch_ch_moe(int mode, int s8, const Fp8ChArgs& a, const Fp8ChMoe& g);
+// the layer quantiser over the expert-sorted rows: row i of x[sorted_pairs[i] / top_k] (sorted_pairs == nullptr: x[i]),
+// dynamic (s_in == nullptr) or with the scale s_in[e] of its expert e (found in offsets [E])
+int launch_ch_moe_gather(int s8, const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in,
+                         int E, void* codes, float* s_x, int rows, int top_k, int K, float ub, int dtype,
+                         cudaStream_t stream);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

@@ -29,6 +29,9 @@ per-expert loop, arranged for the B200 kernels and for tensor parallelism:
   * FP8 W8A16 experts (every w1 / w3 / w2 a post_init'ed B200Fp8QuantLinear): the five launches of the GPTQ grouped path
     on the FP8 instantiations of the grouped small-batch kernels, W the exact b2q_fp8_dequant operand.  Both keep the
     modules working on views into the stacks;
+  * per-channel W8A8 experts (B200ChannelFp8Linear / B200ChannelInt8Linear, dynamic or static activations): the same six
+    launches on the e4m3 or s8 tensor cores (grouped modes of b2q_fp8ch.cu).  `MoEExperts` keeps the loop for them;
+    the grouped path is the subclass `B200ChannelW8A8Experts`;
   * LOOP path (fallback: dense stand-ins in CPU tests, mixed experts, regrouped act-order shards): tokens are sorted by
     expert once, every expert sees one contiguous block of its routed tokens; one host sync per block for the per-expert
     counts, like the reference's loop;
@@ -75,8 +78,11 @@ class MoEExperts(torch.nn.Module):
         # separate small kernel overlaps
         self.fuse_act = False
         self._stack = None
+        self._refusal = None  # why the experts do not qualify, when the stack builder says so
         if grouped is None or grouped:
             self._stack = self._build_stack()
+            if grouped and self._stack is None and self._refusal is not None:
+                raise ValueError(f"{type(self).__name__}(grouped=True): {self._refusal}")
             if grouped and self._stack is None:
                 raise ValueError("MoEExperts(grouped=True): experts must be post_init'ed B200 QuantLinears of one shape / "
                                  "group size, with one kernel bit width (4 or 8) for w1 / w3 and one for w2, the same "
@@ -86,7 +92,8 @@ class MoEExperts(torch.nn.Module):
                                  "B200QqqQuantLinears only (one shape and group kind per role, w1 and w3 alike, an "
                                  "intermediate size that is a multiple of 64, at most 256 experts on one device, no bias "
                                  "or adapters); or post_init'ed B200Fp8QuantLinears only (one shape and scale group per "
-                                 "role, at most 256 experts on one device, no bias or adapters)")
+                                 "role, at most 256 experts on one device, no bias or adapters).  Per-channel W8A8 "
+                                 "experts run grouped through B200ChannelW8A8Experts")
         if fuse and self._stack is None:
             from .qlinear import B200KernelMixin, fuse_siblings
 
@@ -495,3 +502,122 @@ class MoEExperts(torch.nn.Module):
         if self.reduce is not None and out.numel() <= self.reduce.max_elems and out.numel() % 8 == 0:
             return self.reduce(out.contiguous())
         return tp.all_reduce_sum_(out, self.group)
+
+
+class B200ChannelW8A8Experts(MoEExperts):
+    """`MoEExperts` over per-channel / per-tensor W8A8 experts (B200ChannelFp8Linear or B200ChannelInt8Linear) that runs
+    the block on the grouped kernels: align -> gather-and-quantise -> gate|up -> quantise h -> down -> combine, six
+    launches with no host synchronisation (include/b2q.h states the rounding points, those of the per-expert loop).
+
+    The stack qualifies when every w1 / w3 / w2 is a post_init'ed module of one of the two classes, with one activation
+    kind and one ``ub`` across the block, no bias or adapter, one device, w1 / w3 [inter, K] and w2 [Kout, inter] with
+    inter % 128 == 0, at most 256 experts, and (static activations) ``w1.input_scale == w3.input_scale`` for every expert,
+    since both quantise the same gathered rows.  Otherwise ``grouped=None`` keeps the inherited loop and ``grouped=True``
+    raises a ValueError naming the failed condition.  ``ks`` pins the split-K ranks of both grouped GEMMs (0: the
+    heuristic)."""
+
+    ks = 0
+
+    def _w8a8_refusal(self):
+        """None when the experts qualify for the grouped W8A8 kernels, else the reason they do not."""
+        from .fp8_channel import B200ChannelFp8Linear
+        from .int8_channel import B200ChannelInt8Linear
+
+        w1, w3, w2 = list(self.w1), list(self.w3), list(self.w2)
+        every = w1 + w3 + w2
+        cls = type(every[0])
+        if cls not in (B200ChannelFp8Linear, B200ChannelInt8Linear) or any(type(m) is not cls for m in every):
+            return "experts must all be B200ChannelFp8Linear or all B200ChannelInt8Linear modules"
+        if len(w1) > 256:
+            return f"at most 256 experts, got {len(w1)}"
+        if not all(m._ready for m in every):
+            return "every expert module must be post_init'ed"
+        if any(m.bias is not None for m in every):
+            return "expert modules must have no bias"
+        if any(m.adapter for m in every):
+            return "expert modules must have no adapter"
+        if len({m.weight.device for m in every}) != 1:
+            return "expert modules must live on one device"
+        if len({(m.activation, m.ub) for m in every}) != 1:
+            return "every expert module must have the same activation kind and ub"
+        K, inter = w1[0].in_features, w1[0].out_features
+        Kout = w2[0].out_features
+        if any((m.in_features, m.out_features) != (K, inter) for m in w1 + w3):
+            return f"w1 and w3 must all be [{inter}, {K}]"
+        if any((m.in_features, m.out_features) != (inter, Kout) for m in w2):
+            return f"w2 must all be [{Kout}, {inter}]"
+        if inter % 128 != 0:
+            return f"the intermediate size {inter} must be a multiple of 128"
+        if w1[0].activation == "static":
+            for e, (a, b) in enumerate(zip(w1, w3)):
+                if not torch.equal(a.input_scale, b.input_scale):
+                    return f"expert {e}: w1 and w3 quantise the same rows, so their input_scale must be equal"
+        return None
+
+    def _build_stack(self):
+        """Stack the experts' checkpoint tensors (weight [E, N, K], weight_scale [E, N] fp32, static input_scale [E]) once
+        per role; the modules keep views into the stacks.  None (and the reason in `_refusal`) if they do not qualify."""
+        self._refusal = self._w8a8_refusal()
+        if self._refusal is not None:
+            return None
+        from .int8_channel import B200ChannelInt8Linear
+
+        m0 = self.w1[0]
+        out = {"w8a8": True, "int8": isinstance(m0, B200ChannelInt8Linear), "static": m0.activation == "static",
+               "ub": float("inf") if m0.ub is None else m0.ub}
+        for name, mods in (("w1", self.w1), ("w3", self.w3), ("w2", self.w2)):
+            weight = torch.stack([m.weight.view(torch.uint8) for m in mods]).view(m0.CODE_DTYPE)
+            scale = torch.stack([m.weight_scale for m in mods])
+            s_in = torch.cat([m.input_scale.reshape(1) for m in mods]) if out["static"] else None
+            for e, m in enumerate(mods):  # the modules keep working on their own; no second copy of the weights
+                m.weight = weight[e]
+                m.weight_scale = scale[e]
+            out[name] = dict(weight=weight, scale=scale, s_in=s_in, K=mods[0].in_features, N=mods[0].out_features)
+        return out
+
+    def _forward_grouped(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
+        """align -> gather-and-quantise -> gate|up -> quantise h -> down -> combine (include/b2q.h)."""
+        from ._lib import check, lib
+
+        T, top_k = topk_ids.shape
+        rows, E = T * top_k, self.num_experts
+        s1, s3, s2 = self._stack["w1"], self._stack["w3"], self._stack["w2"]
+        K, inter, Kout = s1["K"], s1["N"], s2["N"]
+        self._check_x(x, T, top_k, K, topk_weights, s1["weight"].device)
+        dev, dt = x.device, x.dtype
+        code = 0 if dt == torch.float16 else 1
+        st = torch.cuda.current_stream(dev).cuda_stream
+        int8, static, ks = self._stack["int8"], self._stack["static"], int(self.ks)
+        pre = "b2q_int8ch" if int8 else "b2q_fp8ch"
+        ub = () if int8 else (self._stack["ub"],)  # the FP8 quantisers' amax bound (+inf: none)
+        ids = topk_ids.to(torch.int32).contiguous()
+        wts = topk_weights.to(torch.float32).contiguous()
+        x2 = x.contiguous()
+        if x2.data_ptr() % 16 != 0:
+            x2 = x2.clone()
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        tables = torch.empty(2 * E + rows, dtype=torch.int32, device=dev)
+        counts, offsets, sorted_pairs = tables[:E], tables[E:2 * E], tables[2 * E:]
+        codes = torch.empty((rows, K), dtype=torch.uint8, device=dev)
+        s_x = torch.empty(rows, dtype=torch.float32, device=dev)
+        h = torch.empty((rows, inter), dtype=dt, device=dev)
+        codes_h = torch.empty((rows, inter), dtype=torch.uint8, device=dev)
+        s_h = torch.empty(rows, dtype=torch.float32, device=dev)
+        ypair = torch.empty((rows, Kout), dtype=torch.float32, device=dev)
+        y = torch.empty((T, Kout), dtype=dt, device=dev)
+        active = min(E, rows)
+        gather, gate_up, down = (getattr(lib, f"{pre}_moe_{n}") for n in ("gather", "gate_up", "down"))
+        check(lib.b2q_moe_align(p(ids), T, top_k, E, p(counts), p(offsets), p(sorted_pairs), st), "b2q_moe_align")
+        check(gather(p(x2), p(sorted_pairs), p(offsets), p(s1["s_in"]), E, p(codes), p(s_x), T, top_k, K, *ub, code, st),
+              f"{pre}_moe_gather")
+        check(gate_up(p(codes), p(s_x), p(s1["weight"]), p(s1["scale"]), p(s3["weight"]), p(s3["scale"]), p(h), p(counts),
+                      p(offsets), E, rows, active, K, inter, code, ks, st), f"{pre}_moe_gate_up")
+        if static:  # h is already in sorted order: each row takes its expert's w2 input_scale
+            check(gather(p(h), None, p(offsets), p(s2["s_in"]), E, p(codes_h), p(s_h), rows, 1, inter, *ub, code, st),
+                  f"{pre}_moe_gather")
+        else:
+            check(getattr(lib, f"{pre}_quantize")(p(h), p(codes_h), p(s_h), rows, inter, *ub, code, st), f"{pre}_quantize")
+        check(down(p(codes_h), p(s_h), p(s2["weight"]), p(s2["scale"]), p(counts), p(offsets), p(sorted_pairs), p(wts),
+                   p(ypair), E, rows, active, inter, Kout, code, ks, st), f"{pre}_moe_down")
+        check(lib.b2q_moe_combine(p(ypair), p(y), T, top_k, Kout, code, st), "b2q_moe_combine")
+        return y

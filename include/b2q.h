@@ -441,6 +441,50 @@ int b2q_fp8blk_moe_down(const void* codes_h, const float* s_h, const void* w2, c
                         const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
                         int E, int rows, int active, int K, int N, int dtype, int ks, void* stream);
 
+/* Per-channel W8A8 MoE experts, FP8 (b2q_fp8ch_moe_*) and INT8 (b2q_int8ch_moe_*) (an addition to ABI v8): the
+ * experts' w1 / w3 [E*I, K], w2 [E*H, I] code stacks (each expert's checkpoint weight [N, K], back to back) and their
+ * scale stacks s_w fp32 [E, N] (per-tensor scales broadcast to N), the routing tables of b2q_moe_align.  One block is
+ * six launches with no host synchronisation: b2q_moe_align, b2q_*ch_moe_gather, b2q_*ch_moe_gate_up, the quantiser on
+ * h, b2q_*ch_moe_down, b2q_moe_combine.  The quantiser on h is b2q_*ch_quantize (dynamic) or b2q_*ch_moe_gather with
+ * sorted_pairs = NULL and w2's input scales (static).  For every routed pair (token t, slot j, expert e), with Q the
+ * layer quantiser above and s_in[e] the expert's input_scale (static activations):
+ *   (c, s_x)  = Q(x_t)                            (dynamic: the token's codes; static: with s_in1[e] = s_in3[e])
+ *   g = T(fp32(acc(c, W1_e)) * (s_x * s_w1[e]))   (the layer's y without bias: g and u are the values of the layers)
+ *   u = T(fp32(acc(c, W3_e)) * (s_x * s_w3[e]))
+ *   a = T(silu(g)) (silu(g) = g / (1 + __expf(-g)) in fp32),  h = T(a * u)
+ *   (c_h, s_h) = Q(h)                             (down_proj quantises its own input; static: s_in2[e])
+ *   yp_j = T(fp32(acc(c_h, W2_e)) * (s_h * s_w2[e]))
+ *   y_t  = T(sum_j fp32(w_j * yp_j))              (fp32, slot order, one rounding: b2q_moe_combine)
+ * acc is the k-sum of the dense kernels: exact int32 for INT8 (so every expert's g, u and yp equal b2q_int8ch_mm on its
+ * rows at any split), the per-block fp32 chain for FP8 (each expert's rows run the dense kernel's split-K rank order, so
+ * for a pinned ks its results equal b2q_fp8ch_mm on that expert's rows).  Envelope: K % 128 == 0, N % 64 == 0 (the h
+ * width I also % 128, as the down launch's K), E <= 256, ks <= 8, pointers as for b2q_fp8ch_mm; bad arguments return
+ * -2 before any CUDA work. */
+/* codes [T*top_k, K], s_x fp32 [T*top_k]: sorted row i = Q(x[sorted_pairs[i] / top_k]), or Q(x[i]) of an x already
+ * [T*top_k, K] in sorted order when sorted_pairs is NULL.  s_in NULL: dynamic per-token scales (FP8: amax bounded by
+ * ub > 0, +inf: no bound); else fp32 [E], row i takes the scale of the expert whose rows hold it (offsets [E], E). */
+int b2q_fp8ch_moe_gather(const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in, int E,
+                         void* codes, float* s_x, int T, int top_k, int K, float ub, int dtype, void* stream);
+/* h T [rows, N]: w1 / w3 [E*N, K], s_w1 / s_w3 [E, N], N = the intermediate size; active = experts expected to hold
+ * rows (grid sizing); ks = split-K ranks (1..8), <= 0: the heuristic. */
+int b2q_fp8ch_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                          const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                          int active, int K, int N, int dtype, int ks, void* stream);
+/* ypair fp32 [rows, N]: row pair = w[pair] * yp of sorted row i, pair = sorted_pairs[i]; w2 [E*N, K], K = the
+ * intermediate size. */
+int b2q_fp8ch_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                       const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                       int E, int rows, int active, int K, int N, int dtype, int ks, void* stream);
+/* The INT8 twins: int8 codes and weights, no amax bound. */
+int b2q_int8ch_moe_gather(const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in, int E,
+                          void* codes, float* s_x, int T, int top_k, int K, int dtype, void* stream);
+int b2q_int8ch_moe_gate_up(const void* codes, const float* s_x, const void* w1, const float* s_w1, const void* w3,
+                           const float* s_w3, void* h, const int32_t* counts, const int32_t* offsets, int E, int rows,
+                           int active, int K, int N, int dtype, int ks, void* stream);
+int b2q_int8ch_moe_down(const void* codes_h, const float* s_h, const void* w2, const float* s_w2, const int32_t* counts,
+                        const int32_t* offsets, const int32_t* sorted_pairs, const float* pair_weights, float* ypair,
+                        int E, int rows, int active, int K, int N, int dtype, int ks, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
