@@ -67,6 +67,11 @@ SYMBOLS = {
     "b2q_int8ch_quantize_static": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_int8ch_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "b2q_int8ch_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "b2q_w4afp8_packed_bytes": (_sz, [_i, _i]),
+    "b2q_w4afp8_workspace_bytes": (_sz, [_i, _i]),
+    "b2q_w4afp8_prepack": (_i, [_vp, _vp, _i, _i, _vp]),
+    "b2q_w4afp8_mm": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "b2q_w4afp8_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
     "b2q_fp8blk_moe_gather": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b2q_fp8blk_moe_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),

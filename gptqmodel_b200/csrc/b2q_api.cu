@@ -1,4 +1,5 @@
 // b2q_api.cu — the extern "C" boundary declared in include/b2q.h: argument validation + tier dispatch.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -931,6 +932,88 @@ int b2q_int8ch_forward(const void* x, const void* weight, const float* s_w, cons
   if ((e = check_cuda(e, "b2q_int8ch_forward")) != 0) return e;
   Fp8ChArgs a = {nullptr, codes, s_x, nullptr, weight, s_w, bias, out, M, K, N, dtype, 0, (cudaStream_t)stream};
   return check_cuda(launch_int8ch_gemm(a), "b2q_int8ch_forward");
+}
+
+// ---- W4AFP8 (compressed-tensors W4AFP8: 4-bit group-128 weights, dynamic per-token e4m3 activations) tier ----
+static int w4afp8_check_shape(const char* fn, int M, int K, int N, int dtype) {
+  if (M < 0 || K <= 0 || K % 128 != 0 || K > 65536 || N <= 0 || N % 128 != 0) {
+    set_error("%s: shape M=%d K=%d N=%d outside the envelope (M >= 0, K %% 128 == 0, K <= 65536, N %% 128 == 0)", fn,
+              M, K, N);
+    return -2;
+  }
+  if (dtype != B2Q_DTYPE_F16 && dtype != B2Q_DTYPE_BF16) {
+    set_error("%s: dtype=%d not supported (0 fp16, 1 bf16)", fn, dtype);
+    return -2;
+  }
+  return 0;
+}
+
+static int w4afp8_check_layer(const char* fn, const void* packed, const float* s_w, const void* out) {
+  if (packed == nullptr || s_w == nullptr || out == nullptr) {
+    set_error("%s: null pointer argument", fn);
+    return -2;
+  }
+  if (!aligned16(packed) || !aligned16(s_w) || !aligned16(out)) {
+    set_error("%s: packed, s_w and out must be 16-byte aligned", fn);
+    return -2;
+  }
+  return 0;
+}
+
+size_t b2q_w4afp8_packed_bytes(int K, int N) {
+  if (K <= 0 || K % 128 != 0 || K > 65536 || N <= 0 || N % 128 != 0) return 0;
+  return (size_t)K * N / 2;
+}
+
+size_t b2q_w4afp8_workspace_bytes(int M, int K) { return b2q_fp8ch_workspace_bytes(M, K); }
+
+int b2q_w4afp8_prepack(const int32_t* weight_packed, void* packed, int K, int N, void* stream) {
+  if (int e = w4afp8_check_shape("b2q_w4afp8_prepack", 0, K, N, B2Q_DTYPE_F16)) return e;
+  if (weight_packed == nullptr || packed == nullptr || !aligned16(packed)) {
+    set_error("b2q_w4afp8_prepack: weight_packed and packed (16-byte aligned) must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(packed);
+  return check_cuda(launch_w4afp8_prepack(weight_packed, packed, K, N, (cudaStream_t)stream), "b2q_w4afp8_prepack");
+}
+
+int b2q_w4afp8_mm(const void* codes, const float* s_x, const void* packed, const float* s_w, const void* bias,
+                  void* out, int M, int K, int N, int dtype, int ks, void* stream) {
+  if (int e = w4afp8_check_shape("b2q_w4afp8_mm", M, K, N, dtype)) return e;
+  if (int e = w4afp8_check_layer("b2q_w4afp8_mm", packed, s_w, out)) return e;
+  if (ks > 8) {
+    set_error("b2q_w4afp8_mm: ks=%d exceeds the cluster limit 8", ks);
+    return -2;
+  }
+  if (M == 0) return 0;
+  if (codes == nullptr || s_x == nullptr || !aligned16(codes)) {
+    set_error("b2q_w4afp8_mm: codes (16-byte aligned) and s_x must be device pointers");
+    return -2;
+  }
+  DeviceGuard dg(packed);
+  W4Fp8Args a = {codes, s_x, packed, s_w, bias, out, M, K, N, dtype, ks, (cudaStream_t)stream};
+  return check_cuda(launch_w4afp8_gemm(a), "b2q_w4afp8_mm");
+}
+
+int b2q_w4afp8_forward(const void* x, const void* packed, const float* s_w, const void* bias, void* out, int M, int K,
+                       int N, int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int e = w4afp8_check_shape("b2q_w4afp8_forward", M, K, N, dtype)) return e;
+  if (int e = w4afp8_check_layer("b2q_w4afp8_forward", packed, s_w, out)) return e;
+  if (M == 0) return 0;
+  const size_t need = b2q_w4afp8_workspace_bytes(M, K);
+  if (x == nullptr || !aligned16(x) || workspace == nullptr || !aligned16(workspace) || workspace_bytes < need) {
+    set_error("b2q_w4afp8_forward: x and a workspace of b2q_w4afp8_workspace_bytes(M, K) = %zu bytes (16-byte "
+              "aligned) must be given, got %zu", need, workspace_bytes);
+    return -2;
+  }
+  DeviceGuard dg(packed);
+  uint8_t* codes = reinterpret_cast<uint8_t*>(workspace);
+  float* s_x = reinterpret_cast<float*>(codes + fp8blk_codes_bytes(M, K));
+  int e = check_cuda(launch_fp8ch_quant(x, codes, s_x, M, K, INFINITY, dtype, (cudaStream_t)stream),
+                     "b2q_w4afp8_forward");
+  if (e != 0) return e;
+  W4Fp8Args a = {codes, s_x, packed, s_w, bias, out, M, K, N, dtype, 0, (cudaStream_t)stream};
+  return check_cuda(launch_w4afp8_gemm(a), "b2q_w4afp8_forward");
 }
 
 // ---- block-FP8 MoE experts: the grouped modes of fp8blk_gemm_kernel over the routing tables of b2q_moe_align ----

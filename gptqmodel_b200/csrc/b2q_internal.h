@@ -152,6 +152,20 @@ int launch_ch_moe(int mode, int s8, const Fp8ChArgs& a, const Fp8ChMoe& g);
 int launch_ch_moe_gather(int s8, const void* x, const int32_t* sorted_pairs, const int32_t* offsets, const float* s_in,
                          int E, void* codes, float* s_x, int rows, int top_k, int K, float ub, int dtype,
                          cudaStream_t stream);
+// W4AFP8 tier (b2q_w4afp8.cu): prepacked 4-bit weights with fp32 group-128 scales times the e4m3 codes and token scales of
+// launch_fp8ch_quant (ub = +inf)
+struct W4Fp8Args {
+  const void* codes;      // e4m3 codes [M, K]
+  const float* s_x;       // token scales [M]
+  const void* packed;     // b2q_w4afp8_prepack tiles
+  const float* s_w;       // [K/128, N]
+  const void* bias;       // [N] in the output dtype, or nullptr
+  void* out;              // [M, N]
+  int M, K, N, dtype, ks;  // ks <= 0: heuristic
+  cudaStream_t stream;
+};
+int launch_w4afp8_prepack(const int32_t* weight_packed, void* packed, int K, int N, cudaStream_t stream);
+int launch_w4afp8_gemm(const W4Fp8Args& a);
 int launch_gemv(const MmArgs& a);     // 8-bit, M == 1: CUDA-core fp32-FMA GEMV
 bool gemv_supported(const MmArgs& a);
 int launch_decode(const MmArgs& a);   // 4-bit, M <= 8: mma.sync decode tier

@@ -337,7 +337,7 @@ def _ct_ignores(ignore: tuple, name: str) -> bool:
     return any(re.match(k[3:], name) if k.startswith("re:") else k == name for k in ignore)
 
 
-def _ct_args(where: str, a, kinds, want: str = "float") -> tuple:
+def _ct_args(where: str, a, kinds, want: str = "float", bits: int = 8) -> tuple:
     """(strategy, dynamic) of one compressed-tensors QuantizationArgs dict that this package serves."""
     if not isinstance(a, dict):
         raise ValueError(f"compressed-tensors: `{where}` must be a dict, got {a!r}")
@@ -348,8 +348,8 @@ def _ct_args(where: str, a, kinds, want: str = "float") -> tuple:
         raise ValueError(f"compressed-tensors: `{where}` needs type int | float, a boolean `symmetric` and a `strategy`")
     if not (isinstance(dyn, bool) or dyn == "local"):
         raise ValueError(f"compressed-tensors: `{where}.dynamic` must be a boolean, got {dyn!r}")
-    if typ != want or nb != 8:
-        raise NotImplementedError(f"compressed-tensors: {where} of {nb}-bit {typ} are not served (8-bit {want} only)")
+    if typ != want or nb != bits:
+        raise NotImplementedError(f"compressed-tensors: {where} of {nb}-bit {typ} are not served ({bits}-bit {want} only)")
     if not sym:
         raise NotImplementedError(f"compressed-tensors: asymmetric {where} are not served")
     if strat not in ("tensor", "channel", "group", "block", "token", "tensor_group", "attn_head"):
@@ -364,6 +364,20 @@ def _ct_w8a8(raw: dict, fmt_name: str, want: str) -> tuple:
     """(weight strategy, activation kind, ignore, kv_cache_scheme) of a compressed-tensors W8A8 config whose groups all
     target ["Linear"] with 8-bit `want` (float | int) symmetric weights (channel | tensor, static) and input activations
     (token / dynamic or tensor / static), the same kind in every group."""
+    def kind(gname: str, g: dict) -> tuple:
+        ws, _ = _ct_args(f"{gname}.weights", g["weights"], {("channel", False), ("tensor", False)}, want)
+        _, dyn = _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True), ("tensor", False)},
+                           want)
+        return ws, "dynamic" if dyn else "static"
+
+    (ws, act), ignore, kv = _ct_groups(raw, fmt_name, "W8A8", kind)
+    return ws, act, ignore, kv
+
+
+def _ct_groups(raw: dict, fmt_name: str, scheme: str, kind) -> tuple:
+    """(kind, ignore, kv_cache_scheme) of a compressed-tensors config of format `fmt_name` whose groups all target
+    ["Linear"] with weights and input activations (`scheme`) and no output activations; kind(name, group) checks a
+    group's arguments and returns what it is, which must be the same in every group."""
     fmt = raw.get("format")
     if fmt != fmt_name:
         raise NotImplementedError(f"compressed-tensors: format `{fmt}` is not served ({fmt_name} only)")
@@ -384,11 +398,8 @@ def _ct_w8a8(raw: dict, fmt_name: str, want: str) -> tuple:
         if g.get("output_activations") is not None:
             raise NotImplementedError(f"compressed-tensors: `{gname}` quantises output activations")
         if g.get("weights") is None or g.get("input_activations") is None:
-            raise NotImplementedError(f"compressed-tensors: `{gname}` is not W8A8 (weights and input activations)")
-        ws, _ = _ct_args(f"{gname}.weights", g["weights"], {("channel", False), ("tensor", False)}, want)
-        _, dyn = _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True), ("tensor", False)},
-                           want)
-        kinds.add((ws, "dynamic" if dyn else "static"))
+            raise NotImplementedError(f"compressed-tensors: `{gname}` is not {scheme} (weights and input activations)")
+        kinds.add(kind(gname, g))
     if len(kinds) != 1:
         raise NotImplementedError(f"compressed-tensors: mixed config groups {sorted(kinds)} are not served")
     ignore = raw.get("ignore") or []
@@ -403,8 +414,8 @@ def _ct_w8a8(raw: dict, fmt_name: str, want: str) -> tuple:
     kv = raw.get("kv_cache_scheme")
     if kv is not None and not isinstance(kv, dict):
         raise ValueError(f"compressed-tensors: `kv_cache_scheme` must be a dict, got {kv!r}")
-    (ws, act), = kinds
-    return ws, act, tuple(ignore), kv
+    (k,) = kinds
+    return k, tuple(ignore), kv
 
 
 def parse_fp8_w8a8_config(raw: dict) -> Fp8W8A8Spec:
@@ -456,8 +467,6 @@ def _load_channel_w8a8(path: str, spec, cls, device, dtype, only, post_init) -> 
     """The `<prefix>.weight` + `<prefix>.weight_scale` modules of a per-channel W8A8 checkpoint as `cls` modules (their
     weights of cls.CODE_DTYPE).  A `weight_zero_point` / `input_zero_point` tensor must be all zeros: the kernels are
     symmetric."""
-    from safetensors import safe_open
-
     code = str(cls.CODE_DTYPE).replace("torch.", "")
     wmap = _weight_map(path)
     if only is not None:
@@ -468,18 +477,8 @@ def _load_channel_w8a8(path: str, spec, cls, device, dtype, only, post_init) -> 
         prefixes = [p for p in prefixes if not spec.ignores(p)]
     dev = torch.device(device)
     do_post = (dev.type == "cuda") if post_init is None else post_init
-    handles: Dict[str, object] = {}
-
-    def tensor(name):
-        fn = wmap.get(name)
-        if fn is None:
-            return None
-        if fn not in handles:
-            handles[fn] = safe_open(fn, framework="pt").__enter__()
-        return handles[fn].get_tensor(name)
-
     mods: Dict[str, nn.Module] = {}
-    try:
+    with _TensorReader(wmap) as tensor:
         for prefix in prefixes:
             t = {s: tensor(f"{prefix}.{s}") for s in ("weight", "weight_scale", "input_scale", "bias")}
             if t["weight"] is None or t["weight_scale"] is None:
@@ -501,13 +500,36 @@ def _load_channel_w8a8(path: str, spec, cls, device, dtype, only, post_init) -> 
             mods[prefix] = cls.from_checkpoint_tensors(
                 t["weight"], ws, input_scale=t["input_scale"], bias=t["bias"], activation=spec.activation,
                 ub=spec.ub, device=dev, dtype=dtype, post_init=do_post, name=prefix)
-    finally:
-        for h in handles.values():
+    return mods
+
+
+class _TensorReader:
+    """`with _TensorReader(weight_map) as tensor:` tensor(name) reads a checkpoint tensor (None when absent), opening
+    each safetensors file once; the files are closed on exit."""
+
+    def __init__(self, wmap: Dict[str, str]):
+        self.wmap, self.handles = wmap, {}
+
+    def __enter__(self):
+        return self.tensor
+
+    def tensor(self, name):
+        from safetensors import safe_open
+
+        fn = self.wmap.get(name)
+        if fn is None:
+            return None
+        if fn not in self.handles:
+            self.handles[fn] = safe_open(fn, framework="pt").__enter__()
+        return self.handles[fn].get_tensor(name)
+
+    def __exit__(self, *exc):
+        for h in self.handles.values():
             close = getattr(h, "__exit__", None)
             if close is not None:
                 close(None, None, None)
-        handles.clear()
-    return mods
+        self.handles.clear()
+        return False
 
 
 @dataclass
@@ -555,6 +577,100 @@ def load_int8_w8a8_linears(path: str, device="cuda", dtype: Optional[torch.dtype
 
     spec = parse_int8_w8a8_config(_read_raw_config(path))
     return _load_channel_w8a8(path, spec, B200ChannelInt8Linear, device, dtype, only, post_init)
+
+
+@dataclass
+class W4Fp8Spec:
+    """A compressed-tensors `W4AFP8` config (`pack-quantized`): symmetric 4-bit int weights with group-128 scales and
+    dynamic per-token e4m3 activations.  kv_cache_scheme is returned untouched, as for Fp8W8A8Spec."""
+    ignore: tuple = ()                # names / "re:" patterns
+    kv_cache_scheme: Optional[dict] = None
+
+    def ignores(self, name: str) -> bool:
+        return _ct_ignores(self.ignore, name)
+
+
+def parse_w4afp8_config(raw: dict) -> W4Fp8Spec:
+    """W4AFP8 configs: `quant_method: compressed-tensors`, `format: pack-quantized`; every config group targets
+    ["Linear"] with weights {num_bits: 4, type: int, symmetric: true, dynamic: false, strategy: group, group_size: 128,
+    actorder: null | "weight"} and input activations {num_bits: 8, type: float, symmetric: true, strategy: token,
+    dynamic: true}.  `ignore` holds module names and `re:` patterns.  NotImplementedError for what the kernels do not
+    serve (other group sizes, channel / tensor strategies, other bit widths, asymmetric weights, `actorder: group`,
+    static, per-tensor or int activations, mixed groups, output activations, other targets), ValueError for malformed
+    entries."""
+    if not isinstance(raw, dict):
+        raise ValueError(f"W4AFP8: the quantisation config must be a dict, got {type(raw).__name__}")
+    method = raw.get("quant_method")
+    if method != "compressed-tensors":
+        raise NotImplementedError(f"W4AFP8: quant_method `{method}` is not compressed-tensors")
+
+    def kind(gname: str, g: dict) -> tuple:
+        w = g["weights"]
+        _ct_args(f"{gname}.weights", w, {("group", False)}, "int", 4)
+        gs = w.get("group_size")
+        if not isinstance(gs, int) or isinstance(gs, bool):
+            raise ValueError(f"compressed-tensors: `{gname}.weights.group_size` must be an integer, got {gs!r}")
+        if gs != 128:
+            raise NotImplementedError(f"compressed-tensors: {gname}.weights with group_size {gs} are not served "
+                                      "(128 only)")
+        ao = w.get("actorder")
+        if ao is not None and not isinstance(ao, str):
+            raise ValueError(f"compressed-tensors: `{gname}.weights.actorder` must be a string or null, got {ao!r}")
+        if ao not in (None, "weight"):
+            raise NotImplementedError(f"compressed-tensors: {gname}.weights with actorder `{ao}` are not served "
+                                      "(null or `weight`: the groups stay contiguous)")
+        _ct_args(f"{gname}.input_activations", g["input_activations"], {("token", True)}, "float", 8)
+        return ("group", "dynamic")
+
+    _, ignore, kv = _ct_groups(raw, "pack-quantized", "W4AFP8", kind)
+    return W4Fp8Spec(ignore, kv)
+
+
+@torch.no_grad()
+def load_w4afp8_linears(path: str, device="cuda", dtype: Optional[torch.dtype] = None,
+                        only: Optional[Iterable[str]] = None,
+                        post_init: Optional[bool] = None) -> Dict[str, nn.Module]:
+    """Load every linear of a compressed-tensors W4AFP8 checkpoint into B200W4Fp8Linear modules.
+
+    Modules are the `<prefix>.weight_packed` + `<prefix>.weight_scale` pairs that the config does not ignore; the rest
+    stay dense and are not returned.  A `weight_zero_point` must be all zeros and a `weight_g_idx` must be
+    arange(K) // 128 (NotImplementedError); shapes outside the kernels' envelope raise NotImplementedError, malformed
+    tensors ValueError.
+    only      : optional iterable of module prefixes to load (default: all found)
+    post_init : default True on CUDA devices, False on CPU (tensors only; host tests)
+    """
+    from .w4afp8 import GROUP, B200W4Fp8Linear
+
+    spec = parse_w4afp8_config(_read_raw_config(path))
+    wmap = _weight_map(path)
+    if only is not None:
+        prefixes = list(only)
+    else:
+        sfx = ".weight_packed"
+        prefixes = sorted(n[: -len(sfx)] for n in wmap if n.endswith(sfx) and n[: -len(sfx)] + ".weight_scale" in wmap)
+        prefixes = [p for p in prefixes if not spec.ignores(p)]
+    dev = torch.device(device)
+    do_post = (dev.type == "cuda") if post_init is None else post_init
+    mods: Dict[str, nn.Module] = {}
+    with _TensorReader(wmap) as tensor:
+        for prefix in prefixes:
+            t = {s: tensor(f"{prefix}.{s}") for s in ("weight_packed", "weight_scale", "weight_shape", "bias",
+                                                      "weight_zero_point", "weight_g_idx")}
+            if t["weight_packed"] is None or t["weight_scale"] is None:
+                raise KeyError(f"{prefix}: checkpoint misses weight_packed / weight_scale")
+            z = t["weight_zero_point"]
+            if z is not None and bool((z.to(torch.float32) != 0).any()):
+                raise NotImplementedError(f"{prefix}: a non-zero `weight_zero_point` (asymmetric weights) is not served")
+            g = t["weight_g_idx"]
+            if g is not None:
+                K = int(t["weight_packed"].shape[-1]) * 8
+                if g.dim() != 1 or g.numel() != K or not torch.equal(g.to(torch.int64), torch.arange(K) // GROUP):
+                    raise NotImplementedError(f"{prefix}: a `weight_g_idx` other than arange(K) // 128 (activation "
+                                              "order by group) is not served")
+            mods[prefix] = B200W4Fp8Linear.from_checkpoint_tensors(
+                t["weight_packed"], t["weight_scale"], weight_shape=t["weight_shape"], bias=t["bias"], device=dev,
+                dtype=dtype, post_init=do_post, name=prefix)
+    return mods
 
 
 def _weight_map(path: str) -> Dict[str, str]:

@@ -109,7 +109,12 @@ class MoEExperts(torch.nn.Module):
         from .fp8 import B200Fp8QuantLinear
         from .qqq import B200QqqQuantLinear
 
+        from .w4afp8 import B200W4Fp8Linear
+
         every = [m for mods in (self.w1, self.w3, self.w2) for m in mods]
+        if any(isinstance(m, B200W4Fp8Linear) for m in every):
+            self._refusal = "W4AFP8 experts (B200W4Fp8Linear) have no grouped kernels; they run the per-expert loop"
+            return None
         if all(isinstance(m, B200BlockFp8Linear) for m in every):
             return self._build_fp8blk_stack()
         if all(isinstance(m, B200QqqQuantLinear) for m in every):

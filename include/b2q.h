@@ -413,6 +413,35 @@ int b2q_int8ch_forward(const void* x, const void* weight, const float* s_w, cons
                        void* out, int M, int K, int N, int dtype, void* workspace, size_t workspace_bytes,
                        void* stream);
 
+/* W4AFP8 layers (an addition to ABI v8 that changes no earlier entry point): compressed-tensors `W4AFP8` checkpoints
+ * (`pack-quantized`): symmetric int4 weights q in [-8, 7] with one scale per 128 k, dynamic per-token e4m3 activations,
+ * on the e4m3 tensor cores (b2q_w4afp8.cu).  The arithmetic:
+ *   (c, s_x) = b2q_fp8ch_quantize(x, ub = +inf)   (the FP8_DYNAMIC quantiser, unchanged: the same codes and scales);
+ *   P[m, n, b] = sum over k in block b (128 k = one group) of c[m, k] * q[n, k]  (e4m3 x e4m3 wgmma, fp32 accumulator);
+ *   acc[m, n]  = sum over b of P[m, n, b] * s_w[b, n]: acc = fma(P, s_w, acc) once per k-block, in block order within a
+ *                split-K rank; the ranks' partials are then summed in rank order (rank 0 first);
+ *   y[m, n]    = T(acc[m, n] * s_x[m] + bias[n])  (__fmul_rn, __fadd_rn, one rounding to the output dtype T).
+ * Every int4 value is exact in e4m3 and each group scale is applied exactly once, in fp32, to its k-block's partial.
+ * Envelope: K % 128 == 0, K <= 65536, N % 128 == 0; bad arguments return an error (never a partial result).
+ * Tensors: packed = b2q_w4afp8_packed_bytes(K, N) bytes (16-byte aligned), s_w fp32 [K/128, N] (the checkpoint's
+ * weight_scale [N, K/128] widened and transposed), bias [N] in the output dtype or NULL, out [M, N] fp16 / bf16 (dtype
+ * of x).  For a given ks the output is deterministic. */
+size_t b2q_w4afp8_packed_bytes(int K, int N);
+/* Workspace of b2q_w4afp8_forward for M rows: the e4m3 codes and token scales (= b2q_fp8ch_workspace_bytes). */
+size_t b2q_w4afp8_workspace_bytes(int M, int K);
+/* One-time repack of the checkpoint's weight_packed int32 [N, K/8] (code q + 8 of k in bits 4 (k % 8) of word k / 8)
+ * into the kernel's tile layout, in one device pass. */
+int b2q_w4afp8_prepack(const int32_t* weight_packed, void* packed, int K, int N, void* stream);
+/* out[M, N] from e4m3 codes [M, K] and token scales [M] (b2q_fp8ch_quantize's output).  ks in 1..8 pins the split-K
+ * ranks, ks <= 0 takes the heuristic of b2q_w4afp8_forward. */
+int b2q_w4afp8_mm(const void* codes, const float* s_x, const void* packed, const float* s_w, const void* bias,
+                  void* out, int M, int K, int N, int dtype, int ks, void* stream);
+/* The layer: b2q_fp8ch_quantize (ub = +inf) + b2q_w4afp8_mm (ks <= 0) under programmatic dependent launch, through a
+ * caller workspace of b2q_w4afp8_workspace_bytes(M, K) bytes (16-byte aligned).  M is dispatched inside the library; no
+ * allocation and no host synchronisation, so it can be captured in a CUDA graph. */
+int b2q_w4afp8_forward(const void* x, const void* packed, const float* s_w, const void* bias, void* out, int M, int K,
+                       int N, int dtype, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Block-FP8 MoE experts (an addition to ABI v8): the experts' w1 / w3 [E*I, K], w2 [E*H, I] e4m3 stacks and their scale
  * stacks [E, ceil(N/128), K/128] (each expert's checkpoint tensors, back to back), the routing tables of b2q_moe_align.
  * One block is six launches with no host synchronisation: b2q_moe_align, b2q_fp8blk_moe_gather, b2q_fp8blk_moe_gate_up,
