@@ -22,6 +22,6 @@ from .fp8_block import B200BlockFp8Linear  # noqa: F401
 from .fp8_channel import B200ChannelFp8Linear  # noqa: F401
 from .int8_channel import B200ChannelInt8Linear  # noqa: F401
 from .w4afp8 import B200W4Fp8Linear  # noqa: F401
-from .moe import B200ChannelW8A8Experts, MoEExperts  # noqa: F401
+from .moe import B200ChannelW8A8Experts, MoEExperts, route_grouped_sigmoid, route_softmax_topk  # noqa: F401
 
 __all__ = ["B200QuantLinear", "B200AwqQuantLinear", "B200QqqQuantLinear", "B200Fp8QuantLinear", "B200BlockFp8Linear", "B200ChannelFp8Linear", "B200ChannelInt8Linear", "B200W4Fp8Linear", "B200ChannelW8A8Experts", "MoEExperts", "awq_gemm_to_gptq", "Lora", "fuse_siblings", "SiblingGroup", "lib", "check", "B2QError", "LIB_PATH", "SYMBOLS", "ABI_VERSION"]

@@ -45,6 +45,7 @@ SYMBOLS = {
     "b2q_moe_decode_gate_up": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "b2q_moe_decode_act": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "b2q_moe_decode_down": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "b2q_moe_route": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
     "b2q_qqq_packed_bytes": (_sz, [_i, _i]),
     "b2q_qqq_workspace_bytes": (_sz, [_i, _i]),
     "b2q_qqq_prepack": (_i, [_vp, _vp, _i, _i, _i, _vp]),

@@ -1433,6 +1433,39 @@ int b2q_moe_combine(const float* ypair, void* y, int T, int top_k, int N, int dt
   return check_cuda(launch_moe_combine(ypair, y, T, top_k, N, dtype, (cudaStream_t)stream), "b2q_moe_combine");
 }
 
+int b2q_moe_route(const void* logits, int logits_dtype, const float* bias, int T, int E, int top_k, int scoring,
+                  int n_group, int topk_group, int renormalize, float scale, int32_t* topk_ids, float* topk_weights,
+                  void* stream) {
+  const int max_k = E < 16 ? E : 16;
+  if (T < 0 || E < 1 || E > 256 || top_k < 1 || top_k > max_k || logits_dtype < 0 || logits_dtype > 2 ||
+      (scoring != 0 && scoring != 1)) {
+    set_error("b2q_moe_route: bad argument (T=%d E=%d top_k=%d dtype=%d scoring=%d; 1 <= E <= 256, "
+              "1 <= top_k <= min(E, 16))", T, E, top_k, logits_dtype, scoring);
+    return -2;
+  }
+  if (scoring == 0 && (n_group != 1 || topk_group != 1 || bias != nullptr)) {
+    set_error("b2q_moe_route: softmax routing takes n_group = topk_group = 1 and no bias (got %d, %d, %s)", n_group,
+              topk_group, bias != nullptr ? "a bias" : "no bias");
+    return -2;
+  }
+  if (scoring == 1 && (bias == nullptr || n_group < 1 || E % n_group != 0 || E / n_group < 2 || topk_group < 1 ||
+                       topk_group > n_group || top_k > topk_group * (E / n_group))) {
+    set_error("b2q_moe_route: grouped sigmoid routing needs a bias, n_group dividing E with >= 2 experts per group, "
+              "1 <= topk_group <= n_group and top_k <= topk_group * E / n_group (E=%d n_group=%d topk_group=%d top_k=%d)",
+              E, n_group, topk_group, top_k);
+    return -2;
+  }
+  if (T == 0) return 0;
+  if (logits == nullptr || topk_ids == nullptr || topk_weights == nullptr) {
+    set_error("b2q_moe_route: logits / topk_ids / topk_weights missing");
+    return -2;
+  }
+  DeviceGuard dg(topk_ids);
+  return check_cuda(launch_moe_route(logits, logits_dtype, bias, T, E, top_k, scoring, n_group, topk_group, renormalize,
+                                     scale, topk_ids, topk_weights, (cudaStream_t)stream),
+                    "b2q_moe_route");
+}
+
 // ---- MoE decode: one token through its top_k experts on the decode tier (b2q_decode.cu, DecSets::moe) ---------------------
 int b2q_moe_decode_gate_up(const void* x, const void* packed1, const void* scales1, const int32_t* qzeros1,
                            const void* packed3, const void* scales3, const int32_t* qzeros3, const int32_t* topk_ids,

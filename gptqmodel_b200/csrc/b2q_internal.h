@@ -203,6 +203,9 @@ int launch_moe_decode_gate_up(const MmArgs& a, const void* packed1, const void* 
                               const void* packed3, const void* scales3, const int32_t* qzeros3, const int32_t* ids,
                               int top_k, int E, void* gu);                                      // b2q_decode.cu
 int launch_moe_decode_act(const void* gu, void* h, int top_k, int N, int dtype, cudaStream_t stream);  // b2q_moe.cu
+int launch_moe_route(const void* logits, int dtype, const float* bias, int T, int E, int top_k, int scoring, int n_group,
+                     int topk_group, int renormalize, float scale, int32_t* topk_ids, float* topk_weights,
+                     cudaStream_t stream);  // b2q_moe.cu
 int launch_moe_decode_down(const MmArgs& a, const int32_t* ids, const float* wts, int top_k, int E, int fused_act);  // b2q_decode.cu
 // prefill tier over up to 3 sibling weight sets sharing x (x already permuted)
 int launch_gemm_multi(const MmArgs& a, const void* x, int nsets, const void* const* packed, const void* const* scales,

@@ -14,12 +14,210 @@
 // 8-bit.  Act-order experts were prepacked with their rows in group order, so each expert reads its activations in its
 // own column order: moe_gather_perm_kernel replaces step 2 (xs[i, k'] = x[sorted_pairs[i] / k, P13_e[k']]) and, when w2
 // has act-order, permutes h between steps 3 and 4 (h2[i, k'] = h[i, P2_e[k']]).
+// Ahead of step 1, moe_route_kernel turns router logits [T, E] into the topk_ids / topk_weights those steps read (softmax
+// top-k or DeepSeek-V3 grouped sigmoid; include/b2q.h states the arithmetic and the order of the slots).
 #include "b2q_common.cuh"
 #include "b2q_internal.h"
 
 namespace b2q {
 
 constexpr int MOE_MAX_EXPERTS = 256;
+constexpr int ROUTE_WARPS = 4;  // tokens per CTA of moe_route_kernel
+
+// router logits to fp32, exactly
+__device__ __forceinline__ float route_f32(float v) { return v; }
+__device__ __forceinline__ float route_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float route_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+// (v, i) ranks above (bv, bi): the larger value, ties to the lower index
+__device__ __forceinline__ bool route_better(float v, int i, float bv, int bi) {
+  return v > bv || (v == bv && i < bi);
+}
+
+// One round of a warp arg-max over N values per lane, entry (lane, j) standing for index lane + 32 j.  `ok` has bit j set
+// where entry j may still be chosen.  Every lane returns the winner's index (INT_MAX if nothing was eligible) and value;
+// the winning lane also gets its slot in `slot`.
+template <int N>
+__device__ __forceinline__ int route_argmax(const float (&v)[N], unsigned ok, int lane, float& best, int& slot) {
+  float bv = -INFINITY;
+  int bi = INT_MAX;
+  slot = 0;
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    if (((ok >> j) & 1u) && route_better(v[j], lane + 32 * j, bv, bi)) {  // ascending j: ties keep the lower index
+      bv = v[j];
+      bi = lane + 32 * j;
+      slot = j;
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+    if (route_better(ov, oi, bv, bi)) {
+      bv = ov;
+      bi = oi;
+    }
+  }
+  best = bv;
+  return bi;
+}
+
+// One warp per token; lane l holds experts l, l + 32, ... (NPER = ceil(E / 32) of them) in registers.  Selection scores
+// are the logits (softmax) or c = sigmoid(l) + bias (grouped sigmoid), NaN selected as -inf.  The grouped mode keeps the
+// topk_group groups with the largest sum of their two largest c; experts of the other groups are never chosen.  The
+// group scores need a group's experts side by side, so the warp stages c in its own 1 KB of shared memory (__syncwarp
+// only).  k rounds of arg-max give the slots in descending score, ties to the lower index.
+template <typename T, int NPER>
+__global__ void __launch_bounds__(ROUTE_WARPS * 32)
+    moe_route_kernel(const T* __restrict__ logits, const float* __restrict__ bias, int ntok, int E, int top_k,
+                     int scoring, int n_group, int topk_group, int renormalize, float scale,
+                     int32_t* __restrict__ topk_ids, float* __restrict__ topk_weights) {
+  __shared__ float cs[ROUTE_WARPS][MOE_MAX_EXPERTS];
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int t = blockIdx.x * ROUTE_WARPS + warp;
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // the logits are the previous kernel's output
+  if (t >= ntok) return;
+  const T* row = logits + (size_t)t * E;
+  float sel[NPER], wq[NPER];  // selection score; softmax: logit, sigmoid: s = sigmoid(l)
+  unsigned ok = 0;
+#pragma unroll
+  for (int j = 0; j < NPER; ++j) {
+    const int e = lane + 32 * j;
+    sel[j] = -INFINITY;
+    wq[j] = 0.f;
+    if (e < E) {
+      const float l = route_f32(row[e]);
+      ok |= 1u << j;
+      if (scoring == 0) {
+        sel[j] = l;
+      } else {
+        const float s = 1.f / (1.f + expf(-l));
+        wq[j] = s;
+        sel[j] = s + bias[e];
+      }
+      if (sel[j] != sel[j]) sel[j] = -INFINITY;
+    }
+  }
+  float mx = -INFINITY, denom = 1.f;
+  if (scoring == 0) {  // softmax over all E logits: p_e = expf(l_e - max) / sum
+#pragma unroll
+    for (int j = 0; j < NPER; ++j) mx = fmaxf(mx, sel[j]);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < NPER; ++j)
+      if ((ok >> j) & 1u) sum += expf(sel[j] - mx);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+    denom = sum;
+  } else if (topk_group < n_group) {  // group-limited: keep topk_group groups (all kept: nothing to drop)
+    float* c = cs[warp];
+#pragma unroll
+    for (int j = 0; j < NPER; ++j)
+      if ((ok >> j) & 1u) c[lane + 32 * j] = sel[j];
+    __syncwarp();
+    const int gs = E / n_group;
+    constexpr int GPER = MOE_MAX_EXPERTS / 2 / 32;  // n_group <= E / 2 <= 128 groups, lane l holds l, l + 32, ...
+    float gsc[GPER];
+    unsigned gok = 0;
+#pragma unroll
+    for (int j = 0; j < GPER; ++j) {
+      const int g = lane + 32 * j;
+      gsc[j] = -INFINITY;
+      if (g < n_group) {
+        float a = -INFINITY, b = -INFINITY;  // the two largest c of the group
+        for (int i = g * gs; i < (g + 1) * gs; ++i) {
+          const float v = c[i];
+          if (v > a) {
+            b = a;
+            a = v;
+          } else if (v > b) {
+            b = v;
+          }
+        }
+        gsc[j] = a + b;
+        if (gsc[j] != gsc[j]) gsc[j] = -INFINITY;
+        gok |= 1u << j;
+      }
+    }
+    unsigned long long keep_lo = 0, keep_hi = 0;  // kept groups, bit g
+    for (int r = 0; r < topk_group; ++r) {
+      float bv;
+      int slot;
+      const int g = route_argmax<GPER>(gsc, gok, lane, bv, slot);
+      if (lane == (g & 31)) gok &= ~(1u << slot);
+      if (g < 64) keep_lo |= 1ull << g;
+      else keep_hi |= 1ull << (g - 64);
+    }
+#pragma unroll
+    for (int j = 0; j < NPER; ++j) {
+      const int g = (lane + 32 * j) / gs;
+      const bool kept = g < 64 ? (keep_lo >> g) & 1ull : (keep_hi >> (g - 64)) & 1ull;
+      if (!kept) ok &= ~(1u << j);
+    }
+  }
+  int my_id = 0;
+  float my_w = 0.f, sel_sum = 0.f;
+  for (int r = 0; r < top_k; ++r) {
+    float bv;
+    int slot;
+    const int e = route_argmax<NPER>(sel, ok, lane, bv, slot);
+    const int owner = e & 31;
+    float w;
+    if (scoring == 0) {
+      w = expf(bv - mx) / denom;
+    } else {
+      float mine = 0.f;
+#pragma unroll
+      for (int j = 0; j < NPER; ++j)
+        if (j == slot) mine = wq[j];
+      w = __shfl_sync(0xffffffffu, mine, owner);
+    }
+    if (lane == owner) ok &= ~(1u << slot);
+    sel_sum += w;  // slot order
+    if (lane == r) {
+      my_id = e;
+      my_w = w;
+    }
+  }
+  if (lane < top_k) {
+    if (renormalize) my_w = scoring == 0 ? my_w / sel_sum : my_w / (sel_sum + 1e-20f);
+    topk_ids[(size_t)t * top_k + lane] = my_id;
+    topk_weights[(size_t)t * top_k + lane] = my_w * scale;
+  }
+}
+
+template <typename T>
+static int launch_moe_route_t(const void* logits, const float* bias, int T_, int E, int top_k, int scoring, int n_group,
+                              int topk_group, int renormalize, float scale, int32_t* ids, float* wts,
+                              cudaStream_t stream) {
+  const dim3 grid((T_ + ROUTE_WARPS - 1) / ROUTE_WARPS, 1, 1), block(ROUTE_WARPS * 32, 1, 1);
+  const T* x = (const T*)logits;
+#define B2Q_ROUTE(NP)                                                                                                      \
+  return launch_kernel(moe_route_kernel<T, NP>, grid, block, 0, stream, 0, true, x, bias, T_, E, top_k, scoring, n_group, \
+                       topk_group, renormalize, scale, ids, wts)
+  if (E <= 32) B2Q_ROUTE(1);
+  if (E <= 64) B2Q_ROUTE(2);
+  if (E <= 128) B2Q_ROUTE(4);
+  B2Q_ROUTE(8);
+#undef B2Q_ROUTE
+}
+
+int launch_moe_route(const void* logits, int dtype, const float* bias, int T, int E, int top_k, int scoring, int n_group,
+                     int topk_group, int renormalize, float scale, int32_t* topk_ids, float* topk_weights,
+                     cudaStream_t stream) {
+  if (dtype == 0)
+    return launch_moe_route_t<__half>(logits, bias, T, E, top_k, scoring, n_group, topk_group, renormalize, scale,
+                                      topk_ids, topk_weights, stream);
+  if (dtype == 1)
+    return launch_moe_route_t<__nv_bfloat16>(logits, bias, T, E, top_k, scoring, n_group, topk_group, renormalize, scale,
+                                             topk_ids, topk_weights, stream);
+  return launch_moe_route_t<float>(logits, bias, T, E, top_k, scoring, n_group, topk_group, renormalize, scale, topk_ids,
+                                   topk_weights, stream);
+}
 
 __global__ void __launch_bounds__(256)
     moe_align_kernel(const int32_t* __restrict__ topk_ids, int npairs, int E, int32_t* __restrict__ counts,

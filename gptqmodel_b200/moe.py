@@ -59,6 +59,71 @@ def route_topk(router_logits: torch.Tensor, top_k: int):
     return ids, w
 
 
+_ROUTE_DTYPES = {torch.float16: 0, torch.bfloat16: 1, torch.float32: 2}
+
+
+def _route(logits, bias, top_k, scoring, n_group, topk_group, renormalize, scale, who):
+    """Check the arguments of b2q_moe_route (include/b2q.h) and launch it on the logits' device and current stream."""
+    if not isinstance(logits, torch.Tensor):
+        raise ValueError(f"{who}: logits must be a CUDA tensor, got {type(logits).__name__}")
+    if logits.dtype not in _ROUTE_DTYPES or logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError(f"{who}: logits must be a contiguous [T, E] fp16 / bf16 / fp32 tensor, got "
+                         f"{logits.dtype} {tuple(logits.shape)}")
+    T, E = logits.shape
+    top_k, n_group, topk_group = int(top_k), int(n_group), int(topk_group)
+    if not 1 <= E <= 256 or not 1 <= top_k <= min(E, 16):
+        raise ValueError(f"{who}: need 1 <= E <= 256 and 1 <= top_k <= min(E, 16), got E={E} top_k={top_k}")
+    if bias is not None:
+        if (not isinstance(bias, torch.Tensor) or bias.dtype != torch.float32 or tuple(bias.shape) != (E,)
+                or not bias.is_contiguous() or bias.device != logits.device):
+            raise ValueError(f"{who}: correction_bias must be a contiguous fp32 [{E}] tensor on {logits.device}")
+        if n_group < 1 or E % n_group != 0 or E // n_group < 2 or not 1 <= topk_group <= n_group \
+                or top_k > topk_group * (E // n_group):
+            raise ValueError(f"{who}: need n_group dividing E={E} with >= 2 experts per group, 1 <= topk_group <= "
+                             f"n_group and top_k <= topk_group * E / n_group, got n_group={n_group} "
+                             f"topk_group={topk_group} top_k={top_k}")
+    if not logits.is_cuda:
+        raise ValueError(f"{who}: logits must be a CUDA tensor (there is no CPU routing kernel), got {logits.device}")
+    from ._lib import check, lib
+
+    dev = logits.device
+    ids = torch.empty((T, top_k), dtype=torch.int32, device=dev)
+    w = torch.empty((T, top_k), dtype=torch.float32, device=dev)
+    if T == 0:
+        return ids, w
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream(dev).cuda_stream
+        check(lib.b2q_moe_route(logits.data_ptr(), _ROUTE_DTYPES[logits.dtype], None if bias is None else bias.data_ptr(),
+                                T, E, top_k, scoring, n_group, topk_group, int(bool(renormalize)), float(scale),
+                                ids.data_ptr(), w.data_ptr(), st), "b2q_moe_route")
+    return ids, w
+
+
+def route_softmax_topk(logits: torch.Tensor, top_k: int, renormalize: bool = True, scale: float = 1.0):
+    """Softmax top-k routing (Mixtral, Qwen2/3-MoE with ``norm_topk_prob`` on or off, OLMoE, DBRX) in one kernel.
+
+    logits: CUDA [T, E] fp16 / bf16 / fp32, contiguous, E <= 256; 1 <= top_k <= min(E, 16).  Returns (ids int32 [T, top_k],
+    weights fp32 [T, top_k]) on the logits' device and current stream, ready for ``MoEExperts.forward``:
+    p = softmax(logits) in fp32, the top_k experts by logit, weights p (divided by their sum when ``renormalize``) times
+    ``scale``.  Slots come in descending logit, ties to the lower expert index (include/b2q.h: b2q_moe_route)."""
+    return _route(logits, None, top_k, 0, 1, 1, renormalize, scale, "route_softmax_topk")
+
+
+def route_grouped_sigmoid(logits: torch.Tensor, correction_bias: torch.Tensor, top_k: int, n_group: int, topk_group: int,
+                          renormalize: bool = True, scale: float = 1.0):
+    """Grouped sigmoid routing (DeepSeek-V3/R1: n_group 8, topk_group 4; GLM-4.5 / dots1: n_group 1) in one kernel.
+
+    s = sigmoid(logits), c = s + correction_bias (``e_score_correction_bias``, fp32 [E]); the topk_group groups of E / n_group
+    consecutive experts with the largest sum of their two largest c are kept, and the top_k largest c among their experts
+    are selected (experts of dropped groups are never chosen, as in vLLM's grouped_topk; transformers fills them with 0.0,
+    which differs only when a kept group holds a negative c).  Weights are s (divided by sum + 1e-20 when ``renormalize``)
+    times ``scale`` (``routed_scaling_factor``).  Returns (ids int32 [T, top_k], weights fp32 [T, top_k]); slots come in
+    descending c, ties to the lower index (include/b2q.h: b2q_moe_route)."""
+    if not isinstance(correction_bias, torch.Tensor):
+        raise ValueError("route_grouped_sigmoid: correction_bias must be an fp32 tensor")
+    return _route(logits, correction_bias, top_k, 1, n_group, topk_group, renormalize, scale, "route_grouped_sigmoid")
+
+
 class MoEExperts(torch.nn.Module):
     """``y = sum_k w_k * w2_e( silu(w1_e x) * w3_e x )`` over the top-k experts e of every token."""
 

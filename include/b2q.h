@@ -157,6 +157,27 @@ int b2q_moe_decode_down(const void* h, const void* packed2, const void* scales2,
                         const int32_t* topk_ids, const float* topk_weights, int top_k, int E, int K, int N, int bits,
                         int group_size, int dtype, int fused_act, void* y, void* stream);
 
+/* MoE routing (an addition to ABI v8): router logits [T, E] (contiguous; logits_dtype 0 fp16, 1 bf16, 2 fp32, converted to
+ * fp32 exactly, all arithmetic in fp32) -> topk_ids int32 [T, top_k] and topk_weights fp32 [T, top_k], what b2q_moe_align,
+ * b2q_moe_decode_* and the grouped expert launches read.  One launch (one warp per token, programmatic dependent launch:
+ * it waits before the first logits load), no host synchronisation, CUDA-graph capturable.
+ *   scoring 0, softmax (Mixtral, Qwen2/3-MoE, OLMoE, DBRX): experts are selected on the logits l (softmax is monotonic);
+ *     p_e = expf(l_e - max l) / sum_e' expf(l_e' - max l);  w_j = p_j / sum_sel p  (renormalize) or p_j;  then w_j *= scale.
+ *     n_group = topk_group = 1, bias = NULL.
+ *   scoring 1, grouped sigmoid (DeepSeek-V3/R1: n_group 8, topk_group 4; GLM-4.5 / dots1: n_group 1):
+ *     s_e = 1 / (1 + expf(-l_e)),  c_e = s_e + bias_e  (bias = e_score_correction_bias fp32 [E]);
+ *     group score = the sum of the two largest c of the group's E / n_group consecutive experts; the topk_group best groups
+ *     are kept and the top_k largest c are selected among their experts only: experts of the other groups count as -inf
+ *     (vLLM's grouped_topk, DeepSeek's inference code).  transformers' DeepseekV3MoE fills them with 0.0 instead; the two
+ *     agree unless a kept group holds an expert with c < 0.
+ *     w_j = s_j / (sum_sel s + 1e-20) (renormalize) or s_j;  then w_j *= scale (routed_scaling_factor).
+ * Order: ties break toward the lower index, for groups and experts alike; slot j holds the j-th selection, i.e. slots come
+ * in descending selection score (l or c), ties by lower index.  NaN scores select as -inf.
+ * Envelope (-2 otherwise): 1 <= E <= 256, 1 <= top_k <= min(E, 16); scoring 1: n_group divides E, E / n_group >= 2,
+ * 1 <= topk_group <= n_group, top_k <= topk_group * E / n_group.  T = 0 is a no-op. */
+int b2q_moe_route(const void* logits, int logits_dtype, const float* bias, int T, int E, int top_k, int scoring, int n_group,
+                  int topk_group, int renormalize, float scale, int32_t* topk_ids, float* topk_weights, void* stream);
+
 /* In-place all-reduce(sum) of a small 16-bit vector (n % 8 == 0, n <= max_elems) across `world` <= 8 GPUs of one
  * NVLink domain: the single collective of a row-parallel QuantLinear at decode time (the reference has
  * none).  peer_bufs is a HOST array of `world` device pointers to every rank's symmetric buffer (this rank's included),
